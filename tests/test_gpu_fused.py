@@ -181,6 +181,79 @@ def test_fused_corrupt_streams_fail_like_the_pipeline(oracle):
     good = [i for i in range(12) if i not in mutations]
     exp = _oracle_rollup_matrix(oracle, [blocks[i] for i in good], "rate", start, end, step, window)
     assert np.allclose(res[0][good], exp, rtol=1e-12, atol=0, equal_nan=True)
+    # the same through the incremental aggregate (vmb_eval_rollup_aggr_device): the corrupt series are alone in group 0, the
+    # aggregate of the other groups is the oracle's fold of the good series
+    from rollup_names import AGGR
+    G = 4
+    groups = np.array([0 if i in mutations else 1 + i % (G - 1) for i in range(12)], dtype=np.uint32)
+    rc = vm.promql.get_rollup_configs("rate", start, end, step, window)
+
+    class Buf:
+        def __init__(self, nbytes):
+            self.t = torch.empty(nbytes // 8, dtype=torch.float64, device="cuda")
+            self.ptr = self.t.data_ptr()
+    e_v, e_c = np.zeros((G, P)), np.zeros((G, P))
+    for k, i in enumerate(good):
+        row = np.ascontiguousarray(exp[k])
+        oracle.lib().vmo_aggr_update(AGGR["sum"], e_v[groups[i]].ctypes.data_as(oracle.f64p), e_c[groups[i]].ctypes.data_as(oracle.f64p),
+                                     row.ctypes.data_as(oracle.f64p), P)
+    for g in range(G):
+        oracle.lib().vmo_aggr_finalize(AGGR["sum"], e_v[g].ctypes.data_as(oracle.f64p), e_c[g].ctypes.data_as(oracle.f64p), P)
+    for fused in (True, False):
+        ia = vm.promql.IncrementalAggr("sum", G, P, Buf)
+        ctx.set_fused(fused)
+        with pytest.raises(VmbError) as ei:
+            ia.update_blocks(B, rc, groups)
+        ctx.set_fused(True)
+        assert ei.value.code == -53, fused
+        got = ia.finalize(ctx)
+        assert np.allclose(got[1:], e_v[1:], rtol=1e-12, atol=0, equal_nan=True), fused
+
+
+@pytest.mark.parametrize("entry", ["aggr_device_fused", "aggr_device_unfused", "aggr_host", "rollup_aggr_partial", "topk_candidates"])
+def test_group_id_out_of_range_is_rejected(entry):
+    """a group id >= ngroups is an invalid argument (-50) for every entry point that groups series"""
+    import torch
+    import victoriametrics_b200 as vm
+    from victoriametrics_b200 import VmbError
+    rng = np.random.default_rng(SEED0 + 50)
+    S, G = 8, 3
+    blocks = [blockgen.OBlock(blockgen.gen_timestamps(rng, "regular", 1024, T0), blockgen.gen_values(rng, "counter", 1024), -2, 64, i)
+              for i in range(S)]
+    groups = (np.arange(S) % G).astype(np.uint32)
+    groups[5] = G
+    start, end, step, window = T0 + 300000, T0 + 15000 * 1000, 15000, 300000
+    rc = vm.promql.get_rollup_configs("rate", start, end, step, window)
+    descs, payload = blockgen.to_blockset(blocks)
+    ctx = vm.default_context()
+
+    class Buf:
+        def __init__(self, nbytes):
+            self.t = torch.empty(max(nbytes // 8, 1), dtype=torch.float64, device="cuda")
+            self.ptr = self.t.data_ptr()
+    B = vm.storage.Blocks(descs, payload, ctx)
+    try:
+        with pytest.raises(VmbError) as ei:
+            if entry.startswith("aggr_device"):
+                ctx.set_fused(entry == "aggr_device_fused")
+                try:
+                    vm.promql.IncrementalAggr("sum", G, rc.points, Buf).update_blocks(B, rc, groups)
+                finally:
+                    ctx.set_fused(True)
+            elif entry == "aggr_host":
+                vm.promql.eval_rollup_aggr_host("sum", "rate", descs, payload, groups, G, start, end, step, window, ctx=ctx)
+            elif entry == "rollup_aggr_partial":
+                series, _ = vm.storage.decode_blocks(B)
+                try:
+                    vm.promql.IncrementalAggr("sum", G, rc.points, Buf).update(series, rc, groups)
+                finally:
+                    series.close()
+            else:
+                vals = torch.zeros((S, rc.points), dtype=torch.float64, device="cuda")
+                vm.promql.topk(2, vals.data_ptr(), S, rc.points, Buf, group_ids=groups, ngroups=G, ctx=ctx)
+        assert ei.value.code == -50
+    finally:
+        B.close()
 
 
 def test_fused_unaligned_plain_streams_and_all_varint_widths(oracle):

@@ -6,7 +6,6 @@
 #include <stdio.h>
 #include <string.h>
 #include <stdlib.h>
-#include <time.h>
 
 #include <algorithm>
 #include <vector>
@@ -64,13 +63,17 @@ struct DevBuf {  // grow-only device buffer
     }
 };
 
+// Stages of vmb_ctx_last_stage_ms, numbered as in vmb200.h.  The un-fused path records ctx->ev[s] where stage s begins and
+// ev[ST_FUSED] where the aggregate ends, so stage s spans ev[s] .. ev[s + 1]; eval_fused says which events it records.
+enum Stage { ST_ZSTD, ST_DECODE, ST_PREAMBLE, ST_ROLLUP, ST_AGGR, ST_FUSED, ST__COUNT };
+
 struct vmb_ctx {
     int device = 0;
     cudaStream_t stream = 0;
     uint64_t launches = 0;
     bool timing = false;
-    float stage_ms[6] = {0, 0, 0, 0, 0, 0};
-    cudaEvent_t ev[6] = {0, 0, 0, 0, 0, 0};
+    float stage_ms[ST__COUNT] = {};
+    cudaEvent_t ev[ST__COUNT] = {};
     // scratch (reused across calls)
     DevBuf zseq;  // decoded zstd sequences (8 B each) between k_zstd_seq_decode and k_zstd_seq_exec
     DevBuf zscratch, zlit, zstatus, zjobs, zws, args1, args2, rolled, counters, tmp_out, grp, mheap, mnext;
@@ -96,6 +99,7 @@ struct vmb_blocks {
     uint64_t seq_total = 0;   // zstd sequences over all VMB_ZK_HUF columns (size of the record arena)
     bool needs_lit = false;
     uint32_t n_huf = 0, n_gen = 0, n_bad = 0;
+    uint8_t* d_arrays = nullptr;          // the one allocation of the d_ arrays other than the payload (PlanArrays); nullptr in a view
     uint64_t* d_ser_merge_off = nullptr;  // per series: offset into the merge area, UINT64_MAX = none
     vmb_block_desc* d_descs = nullptr;
     uint8_t* d_payload = nullptr;        // = d_payload_alloc + 64
@@ -159,7 +163,7 @@ extern "C" int vmb_ctx_create(int device, vmb_ctx** out) {
     vmb_ctx* c = new vmb_ctx();
     c->device = device;
     c->fused = getenv("VMB_NO_FUSED") == nullptr;  // A/B switch for profiles
-    for (int i = 0; i < 6; i++) CU(cudaEventCreate(&c->ev[i]));
+    for (cudaEvent_t& e : c->ev) CU(cudaEventCreate(&e));
     CU(cudaHostAlloc(&c->h_pinned, 4096, cudaHostAllocDefault));
     *out = c;
     return VMB_OK;
@@ -176,8 +180,8 @@ extern "C" void vmb_ctx_destroy(vmb_ctx* c) {
     DevBuf* bufs[] = {&c->zscratch, &c->zlit, &c->zstatus, &c->zjobs, &c->zws, &c->args1, &c->args2, &c->rolled,
                       &c->counters, &c->tmp_out, &c->grp, &c->mheap, &c->mnext, &c->zseq, &c->bail, &c->sub_arrays, &c->aggr_state, &c->grp_ids, &c->enc_vals, &c->enc_deltas, &c->enc_out, &c->enc_meta};
     for (DevBuf* b : bufs) b->release();
-    for (int i = 0; i < 6; i++)
-        if (c->ev[i]) cudaEventDestroy(c->ev[i]);
+    for (cudaEvent_t e : c->ev)
+        if (e) cudaEventDestroy(e);
     if (c->h_pinned) cudaFreeHost(c->h_pinned);
     if (c->pipe && c->pipe_destroy) c->pipe_destroy(c->pipe);
     delete c;
@@ -205,7 +209,7 @@ extern "C" int vmb_ctx_synchronize(vmb_ctx* c) {
 }
 extern "C" uint64_t vmb_ctx_launch_count(const vmb_ctx* c) { return c ? c->launches : 0; }
 extern "C" float vmb_ctx_last_stage_ms(const vmb_ctx* c, int stage) {
-    return (c && stage >= 0 && stage < 6) ? c->stage_ms[stage] : 0.f;
+    return (c && stage >= 0 && stage < ST__COUNT) ? c->stage_ms[stage] : 0.f;
 }
 extern "C" int vmb_ctx_enable_stage_timing(vmb_ctx* c, int enable) {
     if (!c) return VMB_ERR_INVALID_ARG;
@@ -364,17 +368,8 @@ static int dev_alloc(T** p, size_t n) {
 extern "C" void vmb_blocks_free(vmb_blocks* b) {
     if (!b) return;
     if (b->ctx) cudaSetDevice(b->ctx->device);
-    cudaFree(b->d_descs);
+    cudaFree(b->d_arrays);
     cudaFree(b->d_payload_alloc);
-    cudaFree(b->d_cols);
-    cudaFree(b->d_row_off);
-    cudaFree(b->d_ser_merge_off);
-    cudaFree(b->d_huf_list);
-    cudaFree(b->d_gen_list);
-    cudaFree(b->d_bad_list);
-    cudaFree(b->d_ser_first);
-    cudaFree(b->d_ser_nblocks);
-    cudaFree(b->d_fused_list);
     delete b;
 }
 extern "C" size_t vmb_blocks_count(const vmb_blocks* b) { return b ? b->nblocks : 0; }
@@ -495,13 +490,72 @@ static int plan_blocks(BlocksPlan& pl, const vmb_block_desc* descs, size_t nbloc
     return 0;
 }
 
-template <class T>
-static int upload_vec(T** dptr, const std::vector<T>& v, cudaStream_t st) {
-    int rc = dev_alloc(dptr, v.size());
-    if (rc) return rc;
-    if (!v.empty()) CU(cudaMemcpyAsync(*dptr, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, st));
-    return 0;
-}
+// The descriptors and the arrays of a BlocksPlan in one buffer (16-byte aligned, in this order), followed by up to three uint32
+// arrays of the caller: packed on the host, copied to the device in one transfer and bound to a vmb_blocks there.
+struct PlanArrays {
+    size_t nblocks, descs, cols, row_off, huf, gen, bad, ser_first, ser_nblocks, ser_merge_off, extra[3], bytes;
+    PlanArrays(const BlocksPlan& pl, size_t nb, size_t n_extra0 = 0, size_t n_extra1 = 0, size_t n_extra2 = 0) : nblocks(nb) {
+        const size_t ns = pl.ser_first.size();
+        size_t o = 0;
+        auto take = [&](size_t n) {
+            const size_t at = o;
+            o = al16(o + n);
+            return at;
+        };
+        descs = take(nb * sizeof(vmb_block_desc));
+        cols = take(2 * nb * sizeof(ColInfo));
+        row_off = take((nb + 1) * sizeof(uint64_t));
+        huf = take(pl.huf.size() * 4);
+        gen = take(pl.gen.size() * 4);
+        bad = take(pl.bad.size() * 4);
+        ser_first = take(ns * 4);
+        ser_nblocks = take(ns * 4);
+        ser_merge_off = take(ns * 8);
+        extra[0] = take(n_extra0 * 4);
+        extra[1] = take(n_extra1 * 4);
+        extra[2] = take(n_extra2 * 4);
+        bytes = o;
+    }
+    // d == nullptr: the caller writes the descriptors at h + descs itself
+    void pack(uint8_t* h, const BlocksPlan& pl, const vmb_block_desc* d) const {
+        auto put = [h](size_t at, const auto& v) {
+            if (!v.empty()) memcpy(h + at, v.data(), v.size() * sizeof(v[0]));
+        };
+        if (d && nblocks) memcpy(h + descs, d, nblocks * sizeof(vmb_block_desc));
+        put(cols, pl.cols);
+        put(row_off, pl.row_off);
+        put(huf, pl.huf);
+        put(gen, pl.gen);
+        put(bad, pl.bad);
+        put(ser_first, pl.ser_first);
+        put(ser_nblocks, pl.ser_nblocks);
+        put(ser_merge_off, pl.ser_merge_off);
+    }
+    // sizes of `pl` and array pointers into the packed copy at d; the payload is the caller's
+    void bind(vmb_blocks* b, uint8_t* d, const BlocksPlan& pl) const {
+        b->nblocks = nblocks;
+        b->nseries = pl.ser_first.size();
+        b->rows = pl.rows;
+        b->compressed = pl.compressed;
+        b->scratch_total = pl.scratch_total;
+        b->merge_rows = pl.merge_rows;
+        b->seq_total = pl.seq_total;
+        b->needs_lit = pl.needs_lit;
+        b->n_huf = (uint32_t)pl.huf.size();
+        b->n_gen = (uint32_t)pl.gen.size();
+        b->n_bad = (uint32_t)pl.bad.size();
+        b->d_descs = (vmb_block_desc*)(d + descs);
+        b->d_cols = (ColInfo*)(d + cols);
+        b->d_row_off = (uint64_t*)(d + row_off);
+        b->d_huf_list = (uint32_t*)(d + huf);
+        b->d_gen_list = (uint32_t*)(d + gen);
+        b->d_bad_list = (uint32_t*)(d + bad);
+        b->d_ser_first = (uint32_t*)(d + ser_first);
+        b->d_ser_nblocks = (uint32_t*)(d + ser_nblocks);
+        b->d_ser_merge_off = (uint64_t*)(d + ser_merge_off);
+    }
+    uint32_t* extra_at(uint8_t* base, int i) const { return (uint32_t*)(base + extra[i]); }
+};
 
 static int blocks_upload_impl(vmb_ctx* ctx, const vmb_block_desc* descs, size_t nblocks, const uint8_t* payload, size_t payload_len,
                               vmb_blocks** out, unsigned long long content_bound) {
@@ -511,65 +565,42 @@ static int blocks_upload_impl(vmb_ctx* ctx, const vmb_block_desc* descs, size_t 
     pl.content_bound = content_bound;
     int rc = plan_blocks(pl, descs, nblocks, payload, payload_len);
     if (rc) return rc;
+    const PlanArrays L(pl, nblocks, pl.fused.size());
+    std::vector<uint8_t> h(L.bytes);
+    L.pack(h.data(), pl, descs);
+    if (!pl.fused.empty()) memcpy(L.extra_at(h.data(), 0), pl.fused.data(), pl.fused.size() * 4);
     vmb_blocks* b = new vmb_blocks();
     b->ctx = ctx;
-    b->nblocks = nblocks;
-    b->nseries = pl.ser_first.size();
-    b->rows = pl.rows;
-    b->compressed = pl.compressed;
-    b->scratch_total = pl.scratch_total;
-    b->merge_rows = pl.merge_rows;
-    b->seq_total = pl.seq_total;
-    b->needs_lit = pl.needs_lit;
-    b->n_huf = (uint32_t)pl.huf.size();
-    b->n_gen = (uint32_t)pl.gen.size();
-    b->n_bad = (uint32_t)pl.bad.size();
-    cudaStream_t st = ctx->stream;
-#define CUB(call)                                                                                  \
-    do {                                                                                           \
-        cudaError_t e_ = (call);                                                                   \
-        if (e_ != cudaSuccess) {                                                                   \
-            vmb_set_error("%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-            vmb_blocks_free(b);                                                                    \
-            return VMB_ERR_CUDA;                                                                   \
-        }                                                                                          \
-    } while (0)
-#define TRY(x)                 \
-    do {                       \
-        int rc_ = (x);         \
-        if (rc_) {             \
-            vmb_blocks_free(b); \
-            return rc_;        \
-        }                      \
-    } while (0)
-    TRY(dev_alloc(&b->d_descs, nblocks));
-    if (nblocks) CUB(cudaMemcpyAsync(b->d_descs, descs, nblocks * sizeof(vmb_block_desc), cudaMemcpyHostToDevice, st));
-    // 64 bytes of slack on both sides: the bitstream windows of zstd.cu read up to 11 bytes before a stream's first byte
-    TRY(dev_alloc(&b->d_payload_alloc, payload_len + 128));
-    b->d_payload = b->d_payload_alloc + 64;
-    CUB(cudaMemsetAsync(b->d_payload_alloc, 0, 64, st));
-    if (payload_len) CUB(cudaMemcpyAsync(b->d_payload, payload, payload_len, cudaMemcpyHostToDevice, st));
-    CUB(cudaMemsetAsync(b->d_payload + payload_len, 0, 64, st));
-    TRY(upload_vec(&b->d_cols, pl.cols, st));
-    TRY(upload_vec(&b->d_row_off, pl.row_off, st));
-    TRY(upload_vec(&b->d_huf_list, pl.huf, st));
-    TRY(upload_vec(&b->d_gen_list, pl.gen, st));
-    TRY(upload_vec(&b->d_bad_list, pl.bad, st));
-    TRY(upload_vec(&b->d_ser_first, pl.ser_first, st));
-    TRY(upload_vec(&b->d_ser_nblocks, pl.ser_nblocks, st));
-    TRY(upload_vec(&b->d_ser_merge_off, pl.ser_merge_off, st));
-    TRY(upload_vec(&b->d_fused_list, pl.fused, st));
-#undef TRY
+    // 64 bytes of slack on both sides of the payload: the bitstream windows of zstd.cu read up to 11 bytes before a stream's first byte
+    rc = dev_alloc(&b->d_arrays, L.bytes);
+    if (!rc) rc = dev_alloc(&b->d_payload_alloc, payload_len + 128);
+    if (!rc) {
+        L.bind(b, b->d_arrays, pl);
+        b->d_fused_list = L.extra_at(b->d_arrays, 0);
+        b->d_payload = b->d_payload_alloc + 64;
+        cudaStream_t st = ctx->stream;
+        cudaError_t e = cudaMemcpyAsync(b->d_arrays, h.data(), L.bytes, cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(b->d_payload_alloc, 0, 64, st);
+        if (e == cudaSuccess && payload_len) e = cudaMemcpyAsync(b->d_payload, payload, payload_len, cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(b->d_payload + payload_len, 0, 64, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);  // `h` goes out of scope
+        if (e != cudaSuccess) {
+            vmb_set_error("uploading %zu blocks: %s", nblocks, cudaGetErrorString(e));
+            rc = VMB_ERR_CUDA;
+        }
+    }
+    if (rc) {
+        vmb_blocks_free(b);
+        return rc;
+    }
     b->h_descs.assign(descs, descs + nblocks);
     b->h_cols = pl.cols;
     b->h_ser_first = pl.ser_first;
     b->h_ser_nblocks = pl.ser_nblocks;
     b->h_fused = pl.fused;
     b->h_unfused = pl.unfused;
-    CUB(cudaStreamSynchronize(st));  // the host vectors go out of scope
     *out = b;
     return VMB_OK;
-#undef CUB
 }
 extern "C" int vmb_blocks_upload(vmb_ctx* ctx, const vmb_block_desc* descs, size_t nblocks, const uint8_t* payload,
                                  size_t payload_len, vmb_blocks** out) {
@@ -700,13 +731,13 @@ static int run_decode(vmb_ctx* ctx, const vmb_blocks* b, vmb_series* s, int64_t 
                       unsigned int* d_failed, bool zstd_done = false, int32_t* d_zstatus_in = nullptr,
                       const uint32_t* d_blk_map = nullptr) {
     cudaStream_t st = ctx->stream;
-    if (ctx->timing && !zstd_done) CU(cudaEventRecord(ctx->ev[0], st));
+    if (ctx->timing && !zstd_done) CU(cudaEventRecord(ctx->ev[ST_ZSTD], st));
     int32_t* d_zstatus = d_zstatus_in;
     if (!zstd_done) {
         int rc = run_zstd(ctx, b, &d_zstatus);
         if (rc) return rc;
     }
-    if (ctx->timing && !zstd_done) CU(cudaEventRecord(ctx->ev[1], st));
+    if (ctx->timing && !zstd_done) CU(cudaEventRecord(ctx->ev[ST_DECODE], st));
     DecodeParams D;
     memset(&D, 0, sizeof(D));
     D.descs = b->d_descs;
@@ -763,7 +794,7 @@ static int run_decode(vmb_ctx* ctx, const vmb_blocks* b, vmb_series* s, int64_t 
         launch_series_dedup(R, st);
         count_launch(ctx);
     }
-    if (ctx->timing && !zstd_done) CU(cudaEventRecord(ctx->ev[2], st));
+    if (ctx->timing && !zstd_done) CU(cudaEventRecord(ctx->ev[ST_PREAMBLE], st));
     CU(cudaGetLastError());
     return 0;
 }
@@ -789,12 +820,45 @@ static int alloc_series_for(vmb_ctx* ctx, const vmb_blocks* b, vmb_series** out)
     return 0;
 }
 
-static int collect_stage_times(vmb_ctx* ctx, int first_ev, int nstages, int first_stage) {
-    if (!ctx->timing) return 0;
-    for (int i = 0; i < nstages; i++) {
-        float ms = 0;
-        CU(cudaEventElapsedTime(&ms, ctx->ev[first_ev + i], ctx->ev[first_ev + i + 1]));
-        ctx->stage_ms[first_stage + i] = ms;
+// stage_ms[stage] = time from ev[from] to ev[to]
+static int stage_span(vmb_ctx* ctx, int stage, int from, int to) {
+    float ms = 0;
+    CU(cudaEventElapsedTime(&ms, ctx->ev[from], ctx->ev[to]));
+    ctx->stage_ms[stage] = ms;
+    return 0;
+}
+// the un-fused stages [first, end) of the last call
+static void collect_stage_times(vmb_ctx* ctx, int first, int end) {
+    if (ctx->timing)
+        for (int s = first; s < end; s++) stage_span(ctx, s, s, s + 1);
+}
+
+// ------------------------------------------------------------------------------------------------ counters
+// ctx->counters holds the counters of one call; the first 16 bytes are copied to the same offsets of ctx->h_pinned, which
+// also takes the fused path's bail count
+enum : size_t { PIN_FAILED = 0, PIN_SCANNED = 8, PIN_COUNTERS_BYTES = 16, PIN_BAIL = 64 };
+struct Counters {
+    unsigned int* d_failed;         // series whose blocks failed to decode
+    unsigned long long* d_scanned;  // samplesScanned
+};
+static int counters_zero(vmb_ctx* ctx, cudaStream_t st, Counters* c) {
+    int rc;
+    if ((rc = ctx->counters.reserve(PIN_COUNTERS_BYTES))) return rc;
+    c->d_failed = (unsigned int*)((char*)ctx->counters.p + PIN_FAILED);
+    c->d_scanned = (unsigned long long*)((char*)ctx->counters.p + PIN_SCANNED);
+    CU(cudaMemsetAsync(ctx->counters.p, 0, PIN_COUNTERS_BYTES, st));
+    return 0;
+}
+// copies the counters back after the work queued on `st` and synchronises it
+static int counters_read(vmb_ctx* ctx, cudaStream_t st, uint64_t* samples_scanned) {
+    char* h = (char*)ctx->h_pinned;
+    CU(cudaMemcpyAsync(h, ctx->counters.p, PIN_COUNTERS_BYTES, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (samples_scanned) *samples_scanned = *(unsigned long long*)(h + PIN_SCANNED);
+    const unsigned int failed = *(unsigned int*)(h + PIN_FAILED);
+    if (failed) {
+        vmb_set_error("%u series hold blocks that failed to decode (see the per-block status)", failed);
+        return VMB_ERR_BLOCK_FAILED;
     }
     return 0;
 }
@@ -819,29 +883,19 @@ extern "C" int vmb_decode_blocks(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_m
     int rc = alloc_series_for(ctx, b, &s);
     if (rc) return rc;
     s->values_are_int = (flags & VMB_DECODE_VALUES_AS_INT64) != 0;
-    if ((rc = ctx->counters.reserve(64))) {
-        vmb_series_free(s);
-        return rc;
-    }
-    unsigned int* d_failed = (unsigned int*)ctx->counters.p;
-    CUS(cudaMemsetAsync(d_failed, 0, 64, ctx->stream), nullptr);
-    rc = run_decode(ctx, b, s, tr_min, tr_max, flags, d_failed);
-    if (rc) {
-        vmb_series_free(s);
-        return rc;
-    }
-    unsigned int* h_failed = (unsigned int*)ctx->h_pinned;
-    CUS(cudaMemcpyAsync(h_failed, d_failed, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream), nullptr);
-    if (block_status && b->nblocks)
+    Counters c;
+    rc = counters_zero(ctx, ctx->stream, &c);
+    if (!rc) rc = run_decode(ctx, b, s, tr_min, tr_max, flags, c.d_failed);
+    if (!rc && block_status && b->nblocks)
         CUS(cudaMemcpyAsync(block_status, s->d_blk_status, b->nblocks * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream), nullptr);
-    CUS(cudaStreamSynchronize(ctx->stream), nullptr);
-    collect_stage_times(ctx, 0, 2, 0);
-    *out = s;
-    if (*h_failed) {
-        vmb_set_error("%u series hold blocks that failed to decode (see the per-block status)", *h_failed);
-        return VMB_ERR_BLOCK_FAILED;
+    if (!rc) rc = counters_read(ctx, ctx->stream, nullptr);
+    if (rc && rc != VMB_ERR_BLOCK_FAILED) {
+        vmb_series_free(s);
+        return rc;
     }
-    return VMB_OK;
+    collect_stage_times(ctx, ST_ZSTD, ST_PREAMBLE);
+    *out = s;
+    return rc;
 }
 
 __global__ void k_meta_from_offsets(SeriesMeta* meta, const uint64_t* offsets, uint32_t n) {
@@ -1239,11 +1293,11 @@ static int run_rollup(vmb_ctx* ctx, vmb_series* s, const vmb_rollup_cfg* cfg, in
     count_launch(ctx);
     if (flags & VMB_RC_DROP_STALE_NANS) s->stale_dropped = true;
     if (flags & VMB_RC_REMOVE_COUNTER_RESETS) s->resets_removed = true;
-    if (ctx->timing && record_events) CU(cudaEventRecord(ctx->ev[3], st));
+    if (ctx->timing && record_events) CU(cudaEventRecord(ctx->ev[ST_ROLLUP], st));
     R.cfg.flags = cfg->flags;
     launch_rollup(R, st);
     count_launch(ctx);
-    if (ctx->timing && record_events) CU(cudaEventRecord(ctx->ev[4], st));
+    if (ctx->timing && record_events) CU(cudaEventRecord(ctx->ev[ST_AGGR], st));
     CU(cudaGetLastError());
     return 0;
 }
@@ -1265,22 +1319,82 @@ extern "C" int vmb_rollup(vmb_ctx* ctx, vmb_series* s, const vmb_rollup_cfg* cfg
         if ((rc = ctx->tmp_out.reserve(total * 8))) return rc;
         d_out = (double*)ctx->tmp_out.p;
     }
-    if ((rc = ctx->counters.reserve(64))) return rc;
-    unsigned long long* d_scanned = (unsigned long long*)((char*)ctx->counters.p + 8);
-    CU(cudaMemsetAsync(d_scanned, 0, 8, ctx->stream));
-    if (ctx->timing) CU(cudaEventRecord(ctx->ev[2], ctx->stream));
-    rc = run_rollup(ctx, s, cfg, points, d_out, d_scanned);
-    if (rc) return rc;
-    unsigned long long* h_scanned = (unsigned long long*)((char*)ctx->h_pinned + 8);
-    CU(cudaMemcpyAsync(h_scanned, d_scanned, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    Counters c;
+    if ((rc = counters_zero(ctx, ctx->stream, &c))) return rc;
+    if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_PREAMBLE], ctx->stream));
+    if ((rc = run_rollup(ctx, s, cfg, points, d_out, c.d_scanned))) return rc;
     if (!out_is_device && total) CU(cudaMemcpyAsync(out, d_out, total * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    collect_stage_times(ctx, 2, 2, 2);
-    if (samples_scanned) *samples_scanned = *h_scanned;
+    if ((rc = counters_read(ctx, ctx->stream, samples_scanned))) return rc;
+    collect_stage_times(ctx, ST_PREAMBLE, ST_AGGR);
     return VMB_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ aggregates
+// CSR of n series by group into caller memory: start[ngroups + 1], order[n] = the series of group g at start[g] ..
+// start[g + 1], ascending (the fold order that keeps sum / avg reproducible bit for bit).  Series i of the batch is series
+// sub[i] of group_ids (i itself without sub).
+static int group_id_error(uint32_t g, size_t series, uint32_t ngroups) {
+    vmb_set_error("group id %u of series %zu out of range (%u groups)", g, series, ngroups);
+    return VMB_ERR_INVALID_ARG;
+}
+static int group_csr(const uint32_t* group_ids, const uint32_t* sub, size_t n, uint32_t ngroups, uint32_t* start, uint32_t* order) {
+    memset(start, 0, ((size_t)ngroups + 1) * 4);
+    for (size_t i = 0; i < n; i++) {
+        const size_t s = sub ? sub[i] : i;
+        if (group_ids[s] >= ngroups) return group_id_error(group_ids[s], s, ngroups);
+        start[group_ids[s] + 1]++;
+    }
+    for (uint32_t g = 0; g < ngroups; g++) start[g + 1] += start[g];
+    std::vector<uint32_t> cur(start, start + ngroups);
+    for (size_t i = 0; i < n; i++) order[cur[group_ids[sub ? sub[i] : i]]++] = (uint32_t)i;
+    return 0;
+}
+// group_csr into ctx->grp (start, order, then `extra` uint32 the caller fills); `h` holds the host copy and must live until the
+// stream is synchronised
+static int upload_group_csr(vmb_ctx* ctx, std::vector<uint32_t>& h, const uint32_t* group_ids, const uint32_t* sub, size_t n,
+                            uint32_t ngroups, size_t extra, uint32_t** d_csr) {
+    h.resize((size_t)ngroups + 1 + n);
+    int rc = group_csr(group_ids, sub, n, ngroups, h.data(), h.data() + ngroups + 1);
+    if (!rc) rc = ctx->grp.reserve((h.size() + extra) * sizeof(uint32_t));
+    if (rc) return rc;
+    *d_csr = (uint32_t*)ctx->grp.p;
+    CU(cudaMemcpyAsync(*d_csr, h.data(), h.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    return 0;
+}
+
+// where an incremental aggregate (evalRollupWithIncrementalAggregate eval.go:1804) folds the rolled-up series: {values,
+// counts}[G x P] in DEVICE memory, by the caller's per-series group ids (host)
+struct AggrTarget {
+    int aggr_id;
+    const uint32_t* group_ids;
+    uint32_t ngroups;
+    double* d_values;
+    double* d_counts;
+};
+static void launch_aggr_merge(vmb_ctx* ctx, cudaStream_t st, int aggr_id, double* dv, double* dc, const double* sv, const double* sc,
+                              size_t n) {
+    k_aggr_merge<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(aggr_id, dv, dc, sv, sc, n);
+    count_launch(ctx);
+}
+// fold the rows `rolled` [series x P] by the group CSR d_csr (upload_group_csr) into t; with d_partial ({values, counts}, 2 x G x P
+// scratch) the fold goes there and is merged into t, otherwise it overwrites t
+static void aggr_fold(vmb_ctx* ctx, cudaStream_t st, const AggrTarget& t, const double* rolled, const uint32_t* d_csr, int64_t points,
+                      double* d_partial) {
+    const size_t cells = (size_t)t.ngroups * (size_t)points;
+    AggrParams A;
+    A.rolled = rolled;
+    A.grp_start = d_csr;
+    A.grp_series = d_csr + t.ngroups + 1;
+    A.values = d_partial ? d_partial : t.d_values;
+    A.counts = d_partial ? d_partial + cells : t.d_counts;
+    A.ngroups = t.ngroups;
+    A.npoints = (uint32_t)points;
+    A.aggr = t.aggr_id;
+    k_aggr_fold<<<(unsigned)((cells + 127) / 128), 128, 0, st>>>(A);
+    count_launch(ctx);
+    if (d_partial) launch_aggr_merge(ctx, st, t.aggr_id, t.d_values, t.d_counts, A.values, A.counts, cells);
+}
+
 extern "C" int vmb_rollup_aggr_partial(vmb_ctx* ctx, vmb_series* s, const vmb_rollup_cfg* cfg, int aggr_id,
                                        const uint32_t* group_ids, uint32_t ngroups, double* d_values, double* d_counts,
                                        double* d_rollup_scratch, uint64_t* samples_scanned) {
@@ -1297,57 +1411,25 @@ extern "C" int vmb_rollup_aggr_partial(vmb_ctx* ctx, vmb_series* s, const vmb_ro
         if ((rc = ctx->rolled.reserve(total * 8))) return rc;
         d_rolled = (double*)ctx->rolled.p;
     }
-    // CSR of series by group (stable: ascending series order inside a group)
-    std::vector<uint32_t> start(ngroups + 1, 0), order(s->nseries);
-    for (size_t i = 0; i < s->nseries; i++) {
-        if (group_ids[i] >= ngroups) return VMB_ERR_INVALID_ARG;
-        start[group_ids[i] + 1]++;
-    }
-    for (uint32_t g = 0; g < ngroups; g++) start[g + 1] += start[g];
-    {
-        std::vector<uint32_t> cur(start.begin(), start.end() - 1);
-        for (size_t i = 0; i < s->nseries; i++) order[cur[group_ids[i]]++] = (uint32_t)i;
-    }
-    size_t gbytes = (ngroups + 1 + s->nseries) * sizeof(uint32_t);
-    if ((rc = ctx->grp.reserve(gbytes))) return rc;
-    uint32_t* d_start = (uint32_t*)ctx->grp.p;
-    uint32_t* d_order = d_start + ngroups + 1;
-    CU(cudaMemcpyAsync(d_start, start.data(), (ngroups + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (s->nseries) CU(cudaMemcpyAsync(d_order, order.data(), s->nseries * 4, cudaMemcpyHostToDevice, st));
-    if ((rc = ctx->counters.reserve(64))) return rc;
-    unsigned long long* d_scanned = (unsigned long long*)((char*)ctx->counters.p + 8);
-    CU(cudaMemsetAsync(d_scanned, 0, 8, st));
-    if (ctx->timing) CU(cudaEventRecord(ctx->ev[2], st));
-    rc = run_rollup(ctx, s, cfg, points, d_rolled, d_scanned);
-    if (rc) return rc;
-    AggrParams A;
-    A.rolled = d_rolled;
-    A.grp_start = d_start;
-    A.grp_series = d_order;
-    A.values = d_values;
-    A.counts = d_counts;
-    A.ngroups = ngroups;
-    A.npoints = (uint32_t)points;
-    A.aggr = aggr_id;
-    uint64_t cells = (uint64_t)ngroups * (uint64_t)points;
-    k_aggr_fold<<<(unsigned)((cells + 127) / 128), 128, 0, st>>>(A);
-    count_launch(ctx);
-    if (ctx->timing) CU(cudaEventRecord(ctx->ev[5], st));
-    unsigned long long* h_scanned = (unsigned long long*)((char*)ctx->h_pinned + 8);
-    CU(cudaMemcpyAsync(h_scanned, d_scanned, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));  // `start`/`order` host vectors go out of scope
-    collect_stage_times(ctx, 2, 3, 2);
-    if (samples_scanned) *samples_scanned = *h_scanned;
+    const AggrTarget t = {aggr_id, group_ids, ngroups, d_values, d_counts};
+    std::vector<uint32_t> h_csr;
+    uint32_t* d_csr;
+    if ((rc = upload_group_csr(ctx, h_csr, group_ids, nullptr, s->nseries, ngroups, 0, &d_csr))) return rc;
+    Counters c;
+    if ((rc = counters_zero(ctx, st, &c))) return rc;
+    if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_PREAMBLE], st));
+    if ((rc = run_rollup(ctx, s, cfg, points, d_rolled, c.d_scanned))) return rc;
+    aggr_fold(ctx, st, t, d_rolled, d_csr, points, nullptr);
+    if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_FUSED], st));
+    if ((rc = counters_read(ctx, st, samples_scanned))) return rc;  // synchronises: `h_csr` goes out of scope
+    collect_stage_times(ctx, ST_PREAMBLE, ST_FUSED);
     return VMB_OK;
 }
 
 extern "C" int vmb_aggr_merge(vmb_ctx* ctx, int aggr_id, double* dv, double* dc, const double* sv, const double* sc, size_t n) {
     if (!ctx || !dv || !dc || !sv || !sc) return VMB_ERR_INVALID_ARG;
     CU(cudaSetDevice(ctx->device));
-    if (n) {
-        k_aggr_merge<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(aggr_id, dv, dc, sv, sc, n);
-        count_launch(ctx);
-    }
+    if (n) launch_aggr_merge(ctx, ctx->stream, aggr_id, dv, dc, sv, sc, n);
     CU(cudaGetLastError());
     return VMB_OK;
 }
@@ -1374,20 +1456,9 @@ extern "C" int vmb_aggr_finalize(vmb_ctx* ctx, int aggr_id, double* dv, const do
 }
 
 // ------------------------------------------------------------------------------------------------ whole path
-// decode + preamble + rollup of one uploaded block set into d_out; no host synchronisation inside
-static int eval_device_async(vmb_ctx* ctx, const vmb_blocks* b, vmb_series* s, int64_t tr_min, int64_t tr_max,
-                             const vmb_rollup_cfg* cfg, int64_t points, double* d_out, unsigned int* d_failed,
-                             unsigned long long* d_scanned) {
-    s->stale_dropped = s->resets_removed = false;
-    s->pre_applied = 0;
-    s->rolled = false;
-    int rc = run_decode(ctx, b, s, tr_min, tr_max, 0, d_failed);
-    if (rc) return rc;
-    return run_rollup(ctx, s, cfg, points, d_out, d_scanned);
-}
-
-// the decoded columns of the one-call device paths: owned by the ctx, grown to the largest batch seen
-static int ctx_column_cache(vmb_ctx* ctx, const vmb_blocks* b, vmb_series** out) {
+// *view = the decoded columns of the one-call device paths, sized to `b`, with no preprocessing applied yet.  The columns are
+// owned by the ctx and grown to the largest batch seen.
+static int column_cache_view(vmb_ctx* ctx, const vmb_blocks* b, vmb_series* view) {
     vmb_series* c = ctx->col_cache;
     if (c && (c->rows < b->rows + b->merge_rows || c->nseries < b->nseries || c->nblocks < b->nblocks)) {
         vmb_series_free(c);
@@ -1398,7 +1469,12 @@ static int ctx_column_cache(vmb_ctx* ctx, const vmb_blocks* b, vmb_series** out)
         if (rc) return rc;
         ctx->col_cache = c;
     }
-    *out = c;
+    *view = *c;
+    view->nseries = b->nseries;
+    view->nblocks = b->nblocks;
+    view->rows = b->rows + b->merge_rows;
+    view->stale_dropped = view->resets_removed = view->rolled = false;
+    view->pre_applied = 0;
     return 0;
 }
 
@@ -1456,71 +1532,41 @@ static bool fused_enabled(const vmb_ctx* ctx, const vmb_blocks* b, const vmb_rol
 // (dense_rows: series sub[i] writes row i of d_out instead of row sub[i])
 static int run_unfused_subset(vmb_ctx* ctx, const vmb_blocks* b, const std::vector<uint32_t>& sub, int32_t* d_zstatus,
                               int64_t tr_min, int64_t tr_max, const vmb_rollup_cfg* cfg, int64_t points, double* d_out,
-                              unsigned int* d_failed, unsigned long long* d_scanned, bool dense_rows = false) {
+                              const Counters& c, bool dense_rows) {
     cudaStream_t st = ctx->stream;
     std::vector<vmb_block_desc> descs;
-    std::vector<ColInfo> cols;
     std::vector<uint32_t> blk_map;
+    BlocksPlan pl;
     for (size_t i = 0; i < sub.size(); i++) {
         const uint32_t fb = b->h_ser_first[sub[i]], nb = b->h_ser_nblocks[sub[i]];
         for (uint32_t k = 0; k < nb; k++) {
             vmb_block_desc d = b->h_descs[fb + k];
             d.series_idx = (uint32_t)i;
             descs.push_back(d);
-            cols.push_back(b->h_cols[2 * (size_t)(fb + k)]);
-            cols.push_back(b->h_cols[2 * (size_t)(fb + k) + 1]);
+            pl.cols.push_back(b->h_cols[2 * (size_t)(fb + k)]);
+            pl.cols.push_back(b->h_cols[2 * (size_t)(fb + k) + 1]);
             blk_map.push_back(fb + k);
         }
     }
     const size_t cn = descs.size(), cs = sub.size();
-    BlocksPlan pl;
     plan_layout(pl, descs.data(), cn);
-    // one staging vector -> one upload
-    size_t o_descs = 0;
-    size_t o_cols = al16(o_descs + cn * sizeof(vmb_block_desc));
-    size_t o_rowoff = al16(o_cols + 2 * cn * sizeof(ColInfo));
-    size_t o_sf = al16(o_rowoff + (cn + 1) * sizeof(uint64_t));
-    size_t o_sn = al16(o_sf + cs * 4);
-    size_t o_mo = al16(o_sn + cs * 4);
-    size_t o_map = al16(o_mo + cs * 8);
-    size_t o_rows = al16(o_map + cn * 4);
-    size_t total = al16(o_rows + cs * 4);
-    std::vector<uint8_t> hs(total);
-    memcpy(hs.data() + o_descs, descs.data(), cn * sizeof(vmb_block_desc));
-    memcpy(hs.data() + o_cols, cols.data(), 2 * cn * sizeof(ColInfo));
-    memcpy(hs.data() + o_rowoff, pl.row_off.data(), (cn + 1) * sizeof(uint64_t));
-    memcpy(hs.data() + o_sf, pl.ser_first.data(), cs * 4);
-    memcpy(hs.data() + o_sn, pl.ser_nblocks.data(), cs * 4);
-    memcpy(hs.data() + o_mo, pl.ser_merge_off.data(), cs * 8);
-    memcpy(hs.data() + o_map, blk_map.data(), cn * 4);
-    memcpy(hs.data() + o_rows, sub.data(), cs * 4);
+    const PlanArrays L(pl, cn, cn, cs);  // extras: block map, output rows
+    std::vector<uint8_t> hs(L.bytes);
+    L.pack(hs.data(), pl, descs.data());
+    memcpy(L.extra_at(hs.data(), 0), blk_map.data(), cn * 4);
+    memcpy(L.extra_at(hs.data(), 1), sub.data(), cs * 4);
     int rc;
-    if ((rc = ctx->sub_arrays.reserve(total + 64))) return rc;
-    CU(cudaMemcpyAsync(ctx->sub_arrays.p, hs.data(), total, cudaMemcpyHostToDevice, st));
+    if ((rc = ctx->sub_arrays.reserve(L.bytes + 64))) return rc;
+    CU(cudaMemcpyAsync(ctx->sub_arrays.p, hs.data(), L.bytes, cudaMemcpyHostToDevice, st));
     uint8_t* da = (uint8_t*)ctx->sub_arrays.p;
     vmb_blocks bv;
     bv.ctx = ctx;
-    bv.nblocks = cn;
-    bv.nseries = cs;
-    bv.rows = pl.rows;
-    bv.merge_rows = pl.merge_rows;
-    bv.d_descs = (vmb_block_desc*)(da + o_descs);
+    L.bind(&bv, da, pl);
     bv.d_payload = b->d_payload;
-    bv.d_cols = (ColInfo*)(da + o_cols);
-    bv.d_row_off = (uint64_t*)(da + o_rowoff);
-    bv.d_ser_first = (uint32_t*)(da + o_sf);
-    bv.d_ser_nblocks = (uint32_t*)(da + o_sn);
-    bv.d_ser_merge_off = (uint64_t*)(da + o_mo);
-    vmb_series* cache = nullptr;
-    if ((rc = ctx_column_cache(ctx, &bv, &cache))) return rc;
-    vmb_series view = *cache;
-    view.nseries = cs;
-    view.nblocks = cn;
-    view.rows = pl.rows + pl.merge_rows;
-    view.stale_dropped = view.resets_removed = false;
-    view.pre_applied = 0;
-    rc = run_decode(ctx, &bv, &view, tr_min, tr_max, 0, d_failed, true, d_zstatus, (const uint32_t*)(da + o_map));
-    if (!rc) rc = run_rollup(ctx, &view, cfg, points, d_out, d_scanned, dense_rows ? nullptr : (const uint32_t*)(da + o_rows), false);
+    vmb_series view;
+    if ((rc = column_cache_view(ctx, &bv, &view))) return rc;
+    rc = run_decode(ctx, &bv, &view, tr_min, tr_max, 0, c.d_failed, true, d_zstatus, L.extra_at(da, 0));
+    if (!rc) rc = run_rollup(ctx, &view, cfg, points, d_out, c.d_scanned, dense_rows ? nullptr : L.extra_at(da, 1), false);
     cudaError_t e = cudaStreamSynchronize(st);  // `hs` goes out of scope
     if (!rc && e != cudaSuccess) {
         vmb_set_error("un-fused sub-batch: %s", cudaGetErrorString(e));
@@ -1529,18 +1575,6 @@ static int run_unfused_subset(vmb_ctx* ctx, const vmb_blocks* b, const std::vect
     return rc;
 }
 
-// decode + preamble + rollup of an uploaded block set into d_out through the fused kernel.  Synchronises the stream once (the
-// bail count has to reach the host); counters (failed series, samplesScanned) are left in the device accumulators.
-// incremental-aggregate sink of the fused path: every series is folded into {values, counts}[G x P] (caller-initialised DEVICE
-// state) instead of being written to a [series x P] matrix
-struct FusedAggr {
-    int aggr_id;
-    const uint32_t* h_group_ids;  // per series of the batch (host)
-    const uint32_t* d_group_ids;  // the same on the device
-    uint32_t ngroups;
-    double* d_values;
-    double* d_counts;
-};
 static bool aggr_fusable(int aggr_id) {
     return aggr_id == VMB_AGGR_SUM || aggr_id == VMB_AGGR_AVG || aggr_id == VMB_AGGR_COUNT || aggr_id == VMB_AGGR_GROUP ||
            aggr_id == VMB_AGGR_SUM2 || aggr_id == VMB_AGGR_MIN || aggr_id == VMB_AGGR_MAX;
@@ -1553,14 +1587,25 @@ __global__ void k_aggr_init(int aggr, double* dv, double* dc, size_t n) {
     dc[i] = 0.0;
 }
 
+// decode + preamble + rollup of an uploaded block set through the fused kernel, into d_out or, with af, folded into af's state
+// (initialised here) instead of written to a [series x P] matrix.  Synchronises the stream once (the bail count has to reach the
+// host); the counters are left on the device.  Events: ev[ST_ZSTD] .. ev[ST_DECODE] the zstd stage, ev[ST_DECODE] ..
+// ev[ST_PREAMBLE] the fused kernel, ev[ST_ROLLUP] .. ev[ST_AGGR] the un-fused sub-batch.
 static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t tr_max, const vmb_rollup_cfg* cfg, int64_t points,
-                      double* d_out, unsigned int* d_failed, unsigned long long* d_scanned, const FusedAggr* af = nullptr) {
+                      double* d_out, const Counters& c, const AggrTarget* af) {
     cudaStream_t st = ctx->stream;
     int rc;
-    if (ctx->timing) CU(cudaEventRecord(ctx->ev[0], st));
+    if (af) {
+        if ((rc = ctx->grp_ids.reserve((b->nseries + 1) * sizeof(uint32_t)))) return rc;
+        CU(cudaMemcpyAsync(ctx->grp_ids.p, af->group_ids, b->nseries * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+        const size_t cells = (size_t)af->ngroups * (size_t)points;
+        k_aggr_init<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(af->aggr_id, af->d_values, af->d_counts, cells);
+        count_launch(ctx);
+    }
+    if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_ZSTD], st));
     int32_t* d_zstatus = nullptr;
     if ((rc = run_zstd(ctx, b, &d_zstatus))) return rc;
-    if (ctx->timing) CU(cudaEventRecord(ctx->ev[1], st));
+    if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_DECODE], st));
     const size_t nf = b->h_fused.size();
     if ((rc = ctx->bail.reserve((nf + 2) * sizeof(uint32_t)))) return rc;
     unsigned int* d_bail_count = (unsigned int*)ctx->bail.p;
@@ -1582,10 +1627,10 @@ static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t
         F.out = (double*)ctx->tmp_out.p;
         F.aggr_values = af->d_values;
         F.aggr_counts = af->d_counts;
-        F.group_ids = af->d_group_ids;
+        F.group_ids = (const uint32_t*)ctx->grp_ids.p;
         F.aggr_id = af->aggr_id;
     }
-    F.scanned = d_scanned;
+    F.scanned = c.d_scanned;
     F.bail_list = d_bail_list;
     F.bail_count = d_bail_count;
     F.nlist = (uint32_t)nf;
@@ -1594,9 +1639,9 @@ static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t
     F.tr_max = tr_max;
     launch_fused(F, st);
     count_launch(ctx);
-    if (ctx->timing) CU(cudaEventRecord(ctx->ev[2], st));
+    if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_PREAMBLE], st));
     CU(cudaGetLastError());
-    unsigned int* h_bail = (unsigned int*)((char*)ctx->h_pinned + 64);
+    unsigned int* h_bail = (unsigned int*)((char*)ctx->h_pinned + PIN_BAIL);
     CU(cudaMemcpyAsync(h_bail, d_bail_count, 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     std::vector<uint32_t> sub(b->h_unfused);
@@ -1607,60 +1652,78 @@ static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t
         std::sort(sub.begin(), sub.end());
     }
     if (ctx->timing) {
-        for (int i = 0; i < 6; i++) ctx->stage_ms[i] = 0.f;
-        float ms = 0;
-        CU(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]));
-        ctx->stage_ms[0] = ms;
-        CU(cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]));
-        ctx->stage_ms[5] = ms;
+        for (float& ms : ctx->stage_ms) ms = 0.f;
+        stage_span(ctx, ST_ZSTD, ST_ZSTD, ST_DECODE);
+        stage_span(ctx, ST_FUSED, ST_DECODE, ST_PREAMBLE);
     }
     if (!sub.empty()) {
-        if (ctx->timing) CU(cudaEventRecord(ctx->ev[3], st));
+        if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_ROLLUP], st));
         if (!af) {
-            if ((rc = run_unfused_subset(ctx, b, sub, d_zstatus, tr_min, tr_max, cfg, points, d_out, d_failed, d_scanned))) return rc;
+            if ((rc = run_unfused_subset(ctx, b, sub, d_zstatus, tr_min, tr_max, cfg, points, d_out, c, false))) return rc;
         } else {
-            // the sub-batch's rows go to a dense scratch matrix, are folded per group (ascending series order) and merged in
+            // the sub-batch's rows go to a dense scratch matrix, are folded per group and merged in
             const size_t cs = sub.size(), cells = (size_t)af->ngroups * (size_t)points;
             if ((rc = ctx->rolled.reserve((cs * (size_t)points + 2 * cells) * 8 + 64))) return rc;
             double* d_rows = (double*)ctx->rolled.p;
-            double* d_pv = d_rows + cs * (size_t)points;
-            double* d_pc = d_pv + cells;
-            if ((rc = run_unfused_subset(ctx, b, sub, d_zstatus, tr_min, tr_max, cfg, points, d_rows, d_failed, d_scanned, true))) return rc;
-            std::vector<uint32_t> start(af->ngroups + 1, 0), order(cs);
-            for (size_t i = 0; i < cs; i++) start[af->h_group_ids[sub[i]] + 1]++;
-            for (uint32_t g = 0; g < af->ngroups; g++) start[g + 1] += start[g];
-            {
-                std::vector<uint32_t> cur(start.begin(), start.end() - 1);
-                for (size_t i = 0; i < cs; i++) order[cur[af->h_group_ids[sub[i]]]++] = (uint32_t)i;
-            }
-            if ((rc = ctx->grp.reserve((af->ngroups + 1 + cs) * sizeof(uint32_t)))) return rc;
-            uint32_t* d_start = (uint32_t*)ctx->grp.p;
-            uint32_t* d_order = d_start + af->ngroups + 1;
-            CU(cudaMemcpyAsync(d_start, start.data(), (af->ngroups + 1) * 4, cudaMemcpyHostToDevice, st));
-            CU(cudaMemcpyAsync(d_order, order.data(), cs * 4, cudaMemcpyHostToDevice, st));
-            AggrParams A;
-            A.rolled = d_rows;
-            A.grp_start = d_start;
-            A.grp_series = d_order;
-            A.values = d_pv;
-            A.counts = d_pc;
-            A.ngroups = af->ngroups;
-            A.npoints = (uint32_t)points;
-            A.aggr = af->aggr_id;
-            k_aggr_fold<<<(unsigned)((cells + 127) / 128), 128, 0, st>>>(A);
-            k_aggr_merge<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(af->aggr_id, af->d_values, af->d_counts, d_pv, d_pc, cells);
-            count_launch(ctx, 2);
-            CU(cudaStreamSynchronize(st));  // `start` / `order` go out of scope
+            if ((rc = run_unfused_subset(ctx, b, sub, d_zstatus, tr_min, tr_max, cfg, points, d_rows, c, true))) return rc;
+            std::vector<uint32_t> h_csr;
+            uint32_t* d_csr;
+            if ((rc = upload_group_csr(ctx, h_csr, af->group_ids, sub.data(), cs, af->ngroups, 0, &d_csr))) return rc;
+            aggr_fold(ctx, st, *af, d_rows, d_csr, points, d_rows + cs * (size_t)points);
+            CU(cudaStreamSynchronize(st));  // `h_csr` goes out of scope
         }
         if (ctx->timing) {
-            CU(cudaEventRecord(ctx->ev[4], st));
+            CU(cudaEventRecord(ctx->ev[ST_AGGR], st));
             CU(cudaStreamSynchronize(st));
-            float ms = 0;
-            CU(cudaEventElapsedTime(&ms, ctx->ev[3], ctx->ev[4]));
-            ctx->stage_ms[1] = ms;  // the un-fused sub-batch as a whole (decode + preamble + rollup)
+            stage_span(ctx, ST_DECODE, ST_ROLLUP, ST_AGGR);  // the un-fused sub-batch as a whole (decode + preamble + rollup)
         }
     }
     return 0;
+}
+
+// decode + preamble + rollup of device-resident blocks into the [series x P] matrix d_out or, with aggr, folded into aggr's state:
+// through the fused kernel where it applies, else through the kernel-per-stage pipeline over the ctx's column cache
+static int eval_device(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t tr_max, const vmb_rollup_cfg* cfg, int64_t points,
+                       double* d_out, const AggrTarget* aggr, uint64_t* samples_scanned) {
+    cudaStream_t st = ctx->stream;
+    const bool fused = fused_enabled(ctx, b, cfg) && (!aggr || aggr_fusable(aggr->aggr_id));
+    int rc;
+    std::vector<uint32_t> h_csr;  // lives until counters_read synchronises
+    uint32_t* d_csr = nullptr;
+    if (aggr && fused) {  // the fused kernel reads the group of every series; group_csr checks only those of the sub-batch
+        for (size_t i = 0; i < b->nseries; i++)
+            if (aggr->group_ids[i] >= aggr->ngroups) return group_id_error(aggr->group_ids[i], i, aggr->ngroups);
+    } else if (aggr) {
+        if ((rc = upload_group_csr(ctx, h_csr, aggr->group_ids, nullptr, b->nseries, aggr->ngroups, 0, &d_csr))) return rc;
+    }
+    Counters c;
+    if ((rc = counters_zero(ctx, st, &c))) return rc;
+    if (fused) {
+        if ((rc = eval_fused(ctx, b, tr_min, tr_max, cfg, points, d_out, c, aggr))) return rc;
+        return counters_read(ctx, st, samples_scanned);
+    }
+    vmb_series view;
+    if ((rc = column_cache_view(ctx, b, &view))) return rc;
+    if ((rc = run_decode(ctx, b, &view, tr_min, tr_max, 0, c.d_failed))) return rc;
+    double* d_rows = d_out;
+    if (aggr) {
+        if ((rc = ctx->rolled.reserve((size_t)b->nseries * (size_t)points * 8))) return rc;
+        d_rows = (double*)ctx->rolled.p;
+    }
+    if ((rc = run_rollup(ctx, &view, cfg, points, d_rows, c.d_scanned))) return rc;
+    if (aggr) {
+        aggr_fold(ctx, st, *aggr, d_rows, d_csr, points, nullptr);
+        if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_FUSED], st));
+    }
+    rc = counters_read(ctx, st, samples_scanned);
+    if (rc && rc != VMB_ERR_BLOCK_FAILED) return rc;
+    if (aggr) {
+        collect_stage_times(ctx, ST_PREAMBLE, ST_FUSED);  // as vmb_rollup_aggr_partial
+    } else if (ctx->timing) {
+        collect_stage_times(ctx, ST_ZSTD, ST_AGGR);
+        ctx->stage_ms[ST_FUSED] = 0.f;
+    }
+    return rc;
 }
 
 extern "C" int vmb_eval_rollup_device(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t tr_max,
@@ -1670,39 +1733,25 @@ extern "C" int vmb_eval_rollup_device(vmb_ctx* ctx, const vmb_blocks* b, int64_t
     int rc = check_cfg(cfg, &points);
     if (rc) return rc;
     CU(cudaSetDevice(ctx->device));
-    if ((rc = ctx->counters.reserve(64))) return rc;
-    unsigned int* d_failed = (unsigned int*)ctx->counters.p;
-    unsigned long long* d_scanned = (unsigned long long*)((char*)ctx->counters.p + 8);
-    CU(cudaMemsetAsync(ctx->counters.p, 0, 64, ctx->stream));
-    if (fused_enabled(ctx, b, cfg)) {
-        if ((rc = eval_fused(ctx, b, tr_min, tr_max, cfg, points, d_out, d_failed, d_scanned))) return rc;
-    } else {
-        vmb_series* cache = nullptr;
-        if ((rc = ctx_column_cache(ctx, b, &cache))) return rc;
-        vmb_series view = *cache;  // shallow view with this batch's logical sizes
-        view.nseries = b->nseries;
-        view.nblocks = b->nblocks;
-        view.rows = b->rows + b->merge_rows;
-        rc = eval_device_async(ctx, b, &view, tr_min, tr_max, cfg, points, d_out, d_failed, d_scanned);
-        if (rc) return rc;
-    }
-    CU(cudaMemcpyAsync(ctx->h_pinned, ctx->counters.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    if (ctx->timing && !fused_enabled(ctx, b, cfg)) {
-        collect_stage_times(ctx, 0, 4, 0);
-        ctx->stage_ms[5] = 0.f;
-    }
-    if (samples_scanned) *samples_scanned = *(unsigned long long*)((char*)ctx->h_pinned + 8);
-    unsigned int failed = *(unsigned int*)ctx->h_pinned;
-    if (failed) {
-        vmb_set_error("%u series hold blocks that failed to decode", failed);
-        return VMB_ERR_BLOCK_FAILED;
-    }
-    return VMB_OK;
+    return eval_device(ctx, b, tr_min, tr_max, cfg, points, d_out, nullptr, samples_scanned);
+}
+
+// decode + preamble + rollup + per-GPU incremental aggregate of device-resident blocks (evalRollupWithIncrementalAggregate
+// eval.go:1804 for one rank)
+extern "C" int vmb_eval_rollup_aggr_device(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t tr_max,
+                                           const vmb_rollup_cfg* cfg, int aggr_id, const uint32_t* group_ids, uint32_t ngroups,
+                                           double* d_values, double* d_counts, uint64_t* samples_scanned) {
+    if (!ctx || !b || !group_ids || !d_values || !d_counts || ngroups == 0 || aggr_id < 0 || aggr_id > VMB_AGGR_GROUP)
+        return VMB_ERR_INVALID_ARG;
+    int64_t points;
+    int rc = check_cfg(cfg, &points);
+    if (rc) return rc;
+    CU(cudaSetDevice(ctx->device));
+    const AggrTarget t = {aggr_id, group_ids, ngroups, d_values, d_counts};
+    return eval_device(ctx, b, tr_min, tr_max, cfg, points, nullptr, &t, samples_scanned);
 }
 
 #include "pipeline.inc"
-#include "aggr_eval.inc"
 #include "topk.inc"
 #include "comm.inc"
 #include "matrix_ops.inc"
