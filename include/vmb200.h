@@ -277,7 +277,9 @@ int vmb_aggr_finalize(vmb_ctx* ctx, int aggr_id, double* d_values, const double*
  *   2. several processes: all-gather the candidate arrays (vmb_topk_allgather: count = cells * kmax * 2 doubles), then
  *      vmb_topk_merge([nparts x cells x kmax] entries, cells = ngroups*P).
  *   3. vmb_topk_apply: ks = one k per point (HOST, getIntK aggr.go:793: NaN / negative -> 0, capped by the group size);
- *      group_sizes = series per group over ALL processes (HOST); row_nonempty = HOST array, 1 byte per series. */
+ *      group_sizes = series per group over ALL processes (HOST); row_nonempty = HOST array, 1 byte per series.
+ *      Every point must satisfy min(floor(ks[p]), largest group size) <= kmax, the kmax the lists were built with (the entry
+ *      that decides a survivor has to be in its list); otherwise VMB_ERR_INVALID_ARG and d_vals is left as it was. */
 int vmb_topk_candidates(vmb_ctx* ctx, const double* d_vals, size_t nseries, size_t points, const uint32_t* group_ids,
                         uint32_t ngroups, uint32_t kmax, int reverse, uint64_t series_id_base, double* d_cand);
 int vmb_topk_merge(vmb_ctx* ctx, const double* d_parts, uint32_t nparts, size_t cells, uint32_t kmax, int reverse, double* d_cand);

@@ -8,6 +8,7 @@ import pytest
 
 import blockgen
 from rollup_names import RF
+from test_gpu_rollup_exact import assert_same_bits
 
 pytestmark = pytest.mark.gpu
 T0 = 1_700_000_000_000
@@ -72,6 +73,5 @@ def test_multi_output_rollups(oracle, name, kw):
             escanned += sc
         exp = np.stack(exp)
         g = got[rc.TagValue]
-        assert np.array_equal(np.isnan(g), np.isnan(exp)), (name, rc.TagValue)
-        assert np.allclose(g, exp, rtol=1e-12, atol=0, equal_nan=True), (name, rc.TagValue)
+        assert_same_bits(g, exp, "%s %s" % (name, rc.TagValue), rc.Func)
     assert gscanned == escanned

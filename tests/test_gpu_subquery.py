@@ -8,6 +8,7 @@ import blockgen
 from conftest import SEED0
 from rollup_names import RF
 from test_baseline_configs import _oracle_rollup_matrix
+from test_gpu_rollup_exact import assert_same_bits
 
 pytestmark = pytest.mark.gpu
 T0 = 1_700_000_000_000
@@ -44,7 +45,7 @@ def test_subquery_outer_rollup_over_device_matrix(oracle, outer, inner):
                                                             step, sq_window, args=args, ctx=ctx)
     # oracle: inner matrix, removeNanValues per row, outer preFunc + Do
     inner_exp = _oracle_rollup_matrix(oracle, blocks, inner, sq_start, sq_end, sq_step, in_window)
-    assert np.allclose(inner_dev.cpu().numpy(), inner_exp, rtol=1e-12, atol=0, equal_nan=True)
+    assert_same_bits(inner_dev.cpu().numpy(), inner_exp, "inner " + inner, inner)
     assert np.isnan(inner_exp).any() and (~np.isnan(inner_exp)).any()
     grid = sq_start + sq_step * np.arange(psq, dtype=np.int64)
     rc = vm.promql.get_rollup_configs(outer, start, end, step, sq_window)
@@ -58,6 +59,5 @@ def test_subquery_outer_rollup_over_device_matrix(oracle, outer, inner):
         exp, sc = oracle.rollup_do(RF[outer], v, t, start, end, step, sq_window, may_adjust_window=rc.MayAdjustWindow,
                                    samples_scanned_per_call=rc.samplesScannedPerCall, args=args)
         total += sc
-        assert np.array_equal(np.isnan(got[s]), np.isnan(exp)), (outer, s)
-        assert np.allclose(got[s], exp, rtol=1e-12, atol=0, equal_nan=True), (outer, s)
+        assert_same_bits(got[s], exp, "%s row %d" % (outer, s), outer)
     assert scanned == total

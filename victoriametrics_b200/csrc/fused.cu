@@ -210,16 +210,20 @@ __device__ __forceinline__ uint32_t compact7(uint32_t w) {
     return (w & 0x7fu) | ((w & 0x7f00u) >> 1) | ((w & 0x7f0000u) >> 2) | ((w & 0x7f000000u) >> 3);
 }
 
-// max / min on a double cell by integer atomics (no NaN operands; -0.0 counts as +0.0).  Non-negative doubles order like signed
-// integers and sit above every negative one; negative doubles order in reverse as unsigned integers and sit above every
-// non-negative one there:   max: v >= 0 -> signed max, v < 0 -> unsigned min;   min: v >= 0 -> signed min, v < 0 -> unsigned max
+// max / min on a double cell by integer atomics (no NaN operands).  Doubles with the sign bit clear order like signed integers
+// and sit above every double with it set; those order in reverse as unsigned integers and sit above every other double there:
+//   max: sign clear -> signed max, set -> unsigned min;   min: sign clear -> signed min, set -> unsigned max.
+// So -0.0 ranks just below +0.0: a cell whose series all give -0.0 keeps -0.0, as the reference's fold does; for a mix of
+// the two zeros the result is the one the reference gets when that zero comes first (its order is scheduling dependent too).
 __device__ __forceinline__ void fu_atomic_max(double* a, double v) {
-    if (v >= 0) atomicMax((long long*)a, __double_as_longlong(v == 0 ? 0.0 : v));
-    else atomicMin((unsigned long long*)a, (unsigned long long)__double_as_longlong(v));
+    const long long b = __double_as_longlong(v);
+    if (b >= 0) atomicMax((long long*)a, b);
+    else atomicMin((unsigned long long*)a, (unsigned long long)b);
 }
 __device__ __forceinline__ void fu_atomic_min(double* a, double v) {
-    if (v >= 0) atomicMin((long long*)a, __double_as_longlong(v == 0 ? 0.0 : v));
-    else atomicMax((unsigned long long*)a, (unsigned long long)__double_as_longlong(v));
+    const long long b = __double_as_longlong(v);
+    if (b >= 0) atomicMin((long long*)a, b);
+    else atomicMax((unsigned long long*)a, (unsigned long long)b);
 }
 // updateAggrSum / Min / Max / Avg / Count / Sum2 (aggr_incremental.go:200-458) for one point of one series: NaN is skipped;
 // the order in which series reach a cell is scheduling dependent, as in the reference (one incrementalAggrContext per worker)
