@@ -64,6 +64,9 @@ int vmb_ctx_set_dedup_interval(vmb_ctx* ctx, int64_t interval_ms);
  * Everything else takes the kernel-per-stage pipeline.  enable = 0 forces that pipeline for every series (default: 1; the
  * environment variable VMB_NO_FUSED sets the default to 0).  Results are bit-identical either way. */
 int vmb_ctx_set_fused(vmb_ctx* ctx, int enable);
+/* CTAs of the fused kernel's (persistent) grid on the current device for rate(): a series list of at most this many series runs
+ * one series per CTA.  Never more than 132 x 5. */
+int vmb_fused_grid(void);
 int vmb_ctx_synchronize(vmb_ctx* ctx);
 const char* vmb_last_error(void);
 int vmb_version(void);

@@ -1481,20 +1481,31 @@ static int column_cache_view(vmb_ctx* ctx, const vmb_blocks* b, vmb_series* view
 // ---- fused path (fused.cu): zstd stage, then ONE kernel per series batch that decodes into shared memory and rolls up; the series
 // it hands back (bail list) and the ones it never takes (multi-block series, other timestamp encodings) go through the un-fused
 // pipeline as a sub-batch that writes the same output rows.
+static const size_t FUSED_SMEM = (sizeof(FusedSmem) + 15) & ~(size_t)15;
+// persistent grid of one instantiation: VMB_SMS x the CTAs per SM the occupancy calculator allows, at most FU_CTAS_PER_SM
+// (eval_fused's tmp_out holds one row per CTA of that many)
+template <typename K>
+static uint32_t fused_grid(K kernel) {
+    int blocks_per_sm = 0;
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FUSED_SMEM);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kernel, FU_THREADS, FUSED_SMEM) != cudaSuccess || blocks_per_sm < 1)
+        blocks_per_sm = 1;
+    if (blocks_per_sm > FU_CTAS_PER_SM) blocks_per_sm = FU_CTAS_PER_SM;
+    return VMB_SMS * (uint32_t)blocks_per_sm;
+}
+
+extern "C" int vmb_fused_grid(void) {
+    static const uint32_t grid = fused_grid(k_fused_rollup<VMB_RF_RATE>);
+    return (int)grid;
+}
+
 static void launch_fused(const FusedParams& P, cudaStream_t st) {
     if (!P.nlist) return;
-    const size_t smem0 = (sizeof(FusedSmem) + 15) & ~(size_t)15;
+    const size_t smem0 = FUSED_SMEM;
 #define FUSED_LAUNCH(KERNEL, SMEM)                                                                                \
     do {                                                                                                          \
-        static int blocks_per_sm = 0;                                                                             \
-        if (!blocks_per_sm) {                                                                                     \
-            cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SMEM));               \
-            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, KERNEL, FU_THREADS, (SMEM)) != cudaSuccess || \
-                blocks_per_sm < 1)                                                                                \
-                blocks_per_sm = 1;                                                                                \
-        }                                                                                                         \
-        uint32_t grid = VMB_SMS * (uint32_t)blocks_per_sm;                                                        \
-        if (grid > P.nlist) grid = P.nlist;                                                                       \
+        static const uint32_t grid0 = fused_grid(KERNEL);                                                         \
+        uint32_t grid = grid0 > P.nlist ? P.nlist : grid0;                                                        \
         KERNEL<<<grid, FU_THREADS, (SMEM), st>>>(P);                                                              \
     } while (0)
     switch (P.cfg.func_id) {  // the value-only functions of BASELINE.json's configs get their own instantiation
@@ -1622,8 +1633,8 @@ static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t
     F.ser_list = b->d_fused_list;
     F.ser_first_block = b->d_ser_first;
     F.out = d_out;
-    if (af) {  // one scratch row per CTA (the grid never exceeds VMB_SMS * 8 CTAs)
-        if ((rc = ctx->tmp_out.reserve((size_t)VMB_SMS * 8 * (size_t)points * 8))) return rc;
+    if (af) {  // one scratch row per CTA (launch_fused caps the grid at VMB_SMS * FU_CTAS_PER_SM CTAs)
+        if ((rc = ctx->tmp_out.reserve((size_t)VMB_SMS * FU_CTAS_PER_SM * (size_t)points * 8))) return rc;
         F.out = (double*)ctx->tmp_out.p;
         F.aggr_values = af->d_values;
         F.aggr_counts = af->d_counts;

@@ -20,13 +20,13 @@
 // do not fit the resident rows -- is handed to the un-fused pipeline through a device-side bail list; the host runs it for
 // exactly those series afterwards (same output rows), so every error code and corner case keeps its one implementation.
 //
-// Decode inside the CTA (8 warps, one 512-byte tile each per fill):
-//   1. every lane takes 16 bytes of its warp's tile, finds the varint terminators (bytes < 0x80); counts are scanned over
+// Decode inside the CTA (4 warps, one 1 KB tile each per fill):
+//   1. every lane takes 2 x 16 bytes of its warp's tile, finds the varint terminators (bytes < 0x80); counts are scanned over
 //      the warp and over the CTA, which gives every lane the row of its first value;
-//   2. a lane decodes the varints whose terminator lies in its 16 bytes (7-bit groups compacted once per lane, then one
+//   2. a lane decodes the varints whose terminator lies in each of its 16-byte groups (7-bit groups compacted once, then one
 //      shift-and-mask per value; the bytes of a varint that starts in the previous 16 bytes are carried in), zig-zag decodes
 //      them, stores them raw at their rows and keeps (count, sum, sum of prefix sums);
-//   3. the triples are combined over the lanes and over the 8 warps -- (s2A + s2B + cntB * s1A) is associative under wrapping
+//   3. the triples are combined over the lanes and over the warps -- (s2A + s2B + cntB * s1A) is associative under wrapping
 //      int64 arithmetic, so the prefix sums are bit-identical to the sequential Go loop; with the counts known from step 1 the
 //      combination is two plain sum scans: s1, then t = s2 + cnt * (exclusive prefix of s1);
 //   4. every lane replays its values with the scanned prefix, converts mantissa -> float64 (decimal.go:100) and overwrites
@@ -34,10 +34,11 @@
 #pragma once
 #include <type_traits>
 
-#define FU_THREADS 256
-#define FU_WARPS 8
+#define FU_THREADS 128
+#define FU_WARPS 4
+#define FU_CTAS_PER_SM 5                  /* __launch_bounds__ minimum: 5 x ~43 KB of shared memory, 96 registers per thread */
 #define FU_CAP 4096                       /* rows of one series resident in shared memory */
-#define FU_G 1                            /* 16-byte groups per lane and fill (2 was measured: the 4096-row ring then takes 6 of 8 tiles per fill and the step gets 5 % slower) */
+#define FU_G 2                            /* 16-byte groups per lane and fill: 4 warps x 32 lanes x 32 bytes = one 4 KB fill */
 #define FU_TILE (512 * FU_G)
 #define FU_FILL (FU_WARPS * FU_TILE)      /* bytes staged per fill */
 #define FU_STAGE (16 + FU_FILL + 16)      /* 16 bytes of the previous tile in front, 16 bytes of padding behind */
@@ -80,6 +81,7 @@ struct FuSeries {
     double dec_e10, dec_rcp;                // Dec (decimal.go:100) of the block's scale
     double rate_D, rate_R;                  // rate(): divisor of a full window and its reciprocal (rate_dt = the span in ms, -1: none)
     int32_t rate_dt, rate_rows, dec_mode;
+    uint32_t s;              // the series (its output row)
     int16_t scale;
     uint8_t bail, is_stream, delta2, do_rcr, stale_matters, lin;
 };
@@ -93,10 +95,13 @@ struct FusedSmem {
     double ev_amt[FU_MAX_EVENTS], ev_cum[FU_MAX_EVENTS];
     uint32_t ev_row[FU_MAX_EVENTS];
     uint32_t nev;
+    unsigned long long nd_v, nd_d1;  // nearest-delta(2) state in front of the next fill: last value, last delta
     uint32_t flags;  // bit 0: bail (set while parsing, read behind the barrier that ends the parse)
     uint32_t flags_emit;  // the same for the emit pass: a word of its own, so that a warp already emitting cannot race a warp still reading `flags`
     unsigned long long s_part[FU_WARPS];
-    FuSeries ser;
+    unsigned long long s_thr[FU_THREADS];  // this thread's share of samplesScanned over the series the CTA finished
+    unsigned long long s_ser[FU_THREADS];  // the same for the current series (dropped when it is handed to the un-fused path)
+    FuSeries ser;  // the current series (read where it is used: it stays valid for the whole series)
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -429,14 +434,40 @@ __device__ void fu_series_setup(const FusedParams& P, uint32_t s, FuSeries* out)
             if (((unsigned long long)__double_as_longlong(o.rate_D) & 0xfffffffffffffull) == 0xfffffffffffffull) o.rate_dt = -1;
         }
     }
+    o.s = s;
     o.bail = bail;
     *out = o;
+}
+
+// Dec (decimal.go:100) of the series' scale, rebuilt from shared memory where it is used
+__device__ __forceinline__ Dec fu_dec(const FuSeries& o) {
+    Dec d;
+    d.e10 = o.dec_e10;
+    d.rcp = o.dec_rcp;
+    d.mode = o.dec_mode;
+    return d;
+}
+
+// stage buffer `bf` <- aligned bytes [fs - 16, fs + FU_FILL) of the stream (clamped to its 16-byte aligned end); one thread
+__device__ __forceinline__ void fu_stage_copy(FusedSmem& S, const uint8_t* A, uint32_t end_al, uint32_t fs, uint32_t bf) {
+    if (fs < end_al) {
+        const uint32_t lo = fs ? fs - 16u : 0u;
+        const uint32_t hi = fs + FU_FILL < end_al ? fs + FU_FILL : end_al;
+        mbar_expect_tx(&S.mbar[bf], hi - lo);
+        bulk_g2s(&S.stage[bf][fs ? 0 : 16], A + lo, hi - lo, &S.mbar[bf]);
+    }
+}
+
+// one thread: series s -> `ser`, and the first fill of its stream (a column the kernel takes) into the idle stage buffer `bf`
+__device__ void fu_series_begin(const FusedParams& P, FusedSmem& S, uint32_t s, FuSeries* ser, uint32_t bf) {
+    fu_series_setup(P, s, ser);
+    if (!ser->bail && ser->is_stream) fu_stage_copy(S, ser->A, ser->end_al, 0, bf);
 }
 
 }  // namespace
 
 template <int F>
-__global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
+__global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(FusedParams P) {
     extern __shared__ __align__(16) unsigned char fu_raw[];
     FusedSmem& S = *reinterpret_cast<FusedSmem*>(fu_raw);
     const FuValsRW RV{S.val};  // RV[absolute row]
@@ -444,8 +475,9 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
     asm volatile("" : "+r"(val_s));  // opaque: kept in a register instead of being rebuilt from the CTA's shared window per access
     const vmb_rollup_cfg& rc = P.cfg;
     const uint32_t tid = threadIdx.x, lane = tid & 31u, w = tid >> 5;
-    unsigned long long scanned_cta = 0;  // this thread's share of samplesScanned over the series the CTA finished
-    uint32_t par0 = 0, par1 = 0;  // mbarrier phase parities of the two stage buffers
+    S.s_thr[tid] = 0;
+    uint32_t par = 0;             // bit b: mbarrier phase parity of stage buffer b (carried over the series)
+    uint32_t buf = 0;             // stage buffer of the next tile; a series starts in the one its predecessor left it at
     if (tid == 0) {
         mbar_init(&S.mbar[0], 1);
         mbar_init(&S.mbar[1], 1);
@@ -455,80 +487,50 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
 
     for (uint32_t li = blockIdx.x; li < P.nlist; li += gridDim.x) {
         __syncthreads();  // the previous series is done with the shared memory
-        const uint32_t s = P.ser_list[li];
-        unsigned long long scanned = 0;  // this series (dropped when the series is handed to the un-fused path)
         if (tid == 0) {
-            fu_series_setup(P, s, &S.ser);
+            fu_series_begin(P, S, P.ser_list[li], &S.ser, buf);
             S.flags = 0;
             S.flags_emit = 0;
             S.nev = 0;
         }
         __syncthreads();
-        bool bail = S.ser.bail != 0;
-        const uint32_t n = S.ser.n;
-        const int64_t dts = S.ser.dts, t_org = S.ser.t_org, window = S.ser.window, max_prev = S.ser.max_prev;
-        const uint8_t* const A = S.ser.A;
-        const uint32_t shift = S.ser.shift, len = S.ser.len, end_al = S.ser.end_al;
-        const bool is_stream = S.ser.is_stream != 0, delta2 = S.ser.delta2 != 0, do_rcr = S.ser.do_rcr != 0;
-        const bool stale_matters = S.ser.stale_matters != 0;
-        const int64_t dconst = S.ser.dconst, first_value = S.ser.first_value;
-        Dec dec;
-        dec.e10 = S.ser.dec_e10;
-        dec.rcp = S.ser.dec_rcp;
-        dec.mode = S.ser.dec_mode;
-        const int32_t dt_row = (int32_t)dts;
-        const float inv_row = 1.0f / (float)dt_row;
-        const int32_t start_r = S.ser.start_r, step32 = S.ser.step32, win32 = S.ser.win32, mpi32 = S.ser.mpi32;
-        const bool lin = S.ser.lin != 0;
-        const int32_t lin_k = S.ser.lin_k, iq0 = S.ser.iq0, jq0 = S.ser.jq0;
+        const FuSeries& SE = S.ser;
+        bool bail = SE.bail != 0;
+        const uint32_t n = SE.n;
+        // what the fill needs is held in registers; what only the points need is read from SE (stays valid for the whole series)
+        // where it is used, so that it is not live through the parse
+        const bool is_stream = SE.is_stream != 0;
+        const int64_t first_value = SE.first_value;
+        const int32_t dt_row = (int32_t)SE.dts;
         const uint32_t nvar = n - 1;
-        const int64_t vlo = (int64_t)shift, vhi = (int64_t)shift + len;  // valid stream positions in aligned coordinates
-        // rate(): the divisor of a full window, its reciprocal (used only when a point's divisor is exactly this one)
-        const int32_t rate_dt = S.ser.rate_dt, rate_rows = S.ser.rate_rows;
-        const double rate_D = S.ser.rate_D, rate_R = S.ser.rate_R;
-        // a previous sample right in front of the window always passes `ts > tStart - maxPrevInterval` when maxPrevInterval >= dt
-        const bool prev_always = mpi32 >= dt_row;
 
-        // stage buffer `bf` <- aligned bytes [fs - 16, fs + FU_FILL) of the stream (clamped to its 16-byte aligned end)
         auto issue_copy = [&](uint32_t fs, uint32_t bf) {
-            if (tid == 0 && fs < end_al) {
-                const uint32_t lo = fs ? fs - 16u : 0u;
-                const uint32_t hi = fs + FU_FILL < end_al ? fs + FU_FILL : end_al;
-                mbar_expect_tx(&S.mbar[bf], hi - lo);
-                bulk_g2s(&S.stage[bf][fs ? 0 : 16], A + lo, hi - lo, &S.mbar[bf]);
-            }
+            if (tid == 0) fu_stage_copy(S, SE.A, SE.end_al, fs, bf);
         };
-        uint32_t fs = 0, buf = 0;          // next unconsumed tile (aligned stream offset), stage buffer holding it
-        bool copy_pending = false;
-        if (!bail && is_stream) {
-            issue_copy(0, 0);
-            copy_pending = true;
-        }
+        uint32_t fs = 0;                   // next unconsumed tile (aligned stream offset); stage[buf] holds it
+        bool copy_pending = !bail && is_stream;  // the first fill is in flight (fu_series_begin)
         // first row (nearest_delta2.go:75 / nearest_delta.go:64: as[0] = firstValue)
         uint32_t N = 0;                    // varints decoded so far
-        uint64_t V = (uint64_t)first_value, D1 = 0;
         uint32_t base = 0, cnt = 0, p = 0;
         uint32_t gen_rows = 0;             // rows produced so far (const / delta-const columns)
         double corr = 0.0, prev_raw = 0.0;
         bool stream_done = !is_stream;
         if (!bail) {
             if (tid == 0) {
-                S.val[0] = dec.conv(first_value);  // (fu_swz(0) == 0)
+                S.val[0] = fu_dec(SE).conv(first_value);  // (fu_swz(0) == 0)
+                S.nd_v = (uint64_t)first_value;
+                S.nd_d1 = 0;
             }
             cnt = 1;
             gen_rows = 1;
         }
-        if (tid == 0) scanned += n;  // samplesScanned starts at len(values) rollup.go:766
+        S.s_ser[tid] = tid == 0 ? n : 0u;  // samplesScanned starts at len(values) rollup.go:766
         __syncthreads();
         if (!bail) prev_raw = S.val[0];
 
         uint32_t guard = 0;
         while (!bail && (p < P.npoints || !stream_done)) {
-            if (++guard > 200000u) {  // every iteration consumes a tile or emits a point: this cannot be reached
-                if (tid == 0) {
-                    printf("fused guard: series %u p %u/%u cnt %u base %u fs %u end_al %u N %u nvar %u stream_done %d is_stream %d gen_rows %u n %u\n", s, p,
-                           P.npoints, cnt, base, fs, end_al, N, nvar, (int)stream_done, (int)is_stream, gen_rows, n);
-                }
+            if (++guard > 200000u) {  // every iteration consumes a tile or emits a point: this cannot be reached (the pipeline takes it)
                 bail = true;
                 break;
             }
@@ -537,11 +539,14 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
             bool progressed = false;
             if (is_stream && !stream_done) {
                 if (copy_pending) {
-                    mbar_wait(&S.mbar[buf], buf ? par1 : par0);
-                    if (buf) par1 ^= 1u; else par0 ^= 1u;
+                    mbar_wait(&S.mbar[buf], (par >> buf) & 1u);
+                    par ^= 1u << buf;
                     copy_pending = false;
                 }
                 const uint8_t* st = &S.stage[buf][16];  // aligned stream byte `fs` sits at st[0]
+                const uint32_t end_al = SE.end_al;
+                const int64_t vlo = (int64_t)SE.shift, vhi = vlo + SE.len;  // valid stream positions in aligned coordinates
+                const bool delta2 = SE.delta2 != 0, do_rcr = SE.do_rcr != 0, stale_matters = SE.stale_matters != 0;
                 const uint32_t off = w * FU_TILE + lane * (16u * FU_G);
                 const int64_t g0 = (int64_t)fs + off;
                 uint32_t t_own[FU_G], vm[FU_G], tm[FU_G], pbm[FU_G];
@@ -586,7 +591,7 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
                 // whole tiles that fit the resident rows (pass-through once the points are done: rows are only validated)
                 const bool discard = p >= P.npoints;
                 if (discard) { cnt = 1; cnt_old = 1; }  // rows are not needed any more: decode over the same ring slots
-                // lane k < 8 holds the count of warp k; inclusive scan over those lanes; a tile fits when the rows before it and its own
+                // lane k < FU_WARPS holds the count of warp k; inclusive scan over those lanes; a tile fits when the rows before it and its own
                 // fit the ring; K = the leading tiles that fit
                 uint32_t K, tot, rb;
                 {
@@ -597,8 +602,8 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
                         const uint32_t u = __shfl_up_sync(VMB_FULL, ic, o);
                         if (lane >= (uint32_t)o) ic += u;
                     }
-                    const uint32_t fits = __ballot_sync(VMB_FULL, lane < FU_WARPS && cnt + ic <= FU_CAP) & 0xffu;
-                    K = (uint32_t)__ffs((int)(~fits & 0x1ffu)) - 1u;  // number of leading ones
+                    const uint32_t fits = __ballot_sync(VMB_FULL, lane < FU_WARPS && cnt + ic <= FU_CAP) & ((1u << FU_WARPS) - 1u);
+                    K = (uint32_t)__ffs((int)(~fits & ((2u << FU_WARPS) - 1u))) - 1u;  // number of leading ones
                     tot = K ? __shfl_sync(VMB_FULL, ic, (int)K - 1) : 0u;
                     const uint32_t ex = __shfl_sync(VMB_FULL, ic - t, (int)(w < FU_WARPS ? w : 0));
                     rb = w < K ? ex : 0u;
@@ -755,7 +760,7 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
                     __syncthreads();
                     if (S.flags & 1u) bail = true;
                     // exclusive prefix over the warps in front, and the totals of the fill: lane k < K holds warp k's triple, one
-                    // 8-lane scan, warp w picks lane w - 1 (prefix) and everybody lane K - 1 (totals)
+                    // FU_WARPS-lane scan, warp w picks lane w - 1 (prefix) and everybody lane K - 1 (totals)
                     uint32_t pc, tc;
                     uint64_t ps1, ps2, ts1, ts2;
                     {
@@ -798,9 +803,11 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
                         const uint32_t fcnt = pc + ecnt;
                         const uint64_t fs1 = ps1 + es1;
                         const uint64_t fs2 = ps2 + es2 + (uint64_t)ecnt * ps1;
+                        const uint64_t V = S.nd_v, D1 = S.nd_d1;
                         uint64_t d1 = D1 + fs1;
                         uint64_t v = delta2 ? (V + fs2 + (uint64_t)fcnt * D1) : (V + fs1);
                         bool saw_stale = false;
+                        const Dec dec = fu_dec(SE);
                         auto emit_run = [&](auto is_delta2) {
                             constexpr bool D2 = decltype(is_delta2)::value;
                             for (uint32_t k = 0; k < cl; k++) {
@@ -837,12 +844,17 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
                         else emit_run(std::false_type{});
                         if (saw_stale && stale_matters) S.flags_emit = 1u;
                     }
-                    // ---- carries
-                    if (delta2) {
-                        V += ts2 + (uint64_t)tc * D1;
-                        D1 += ts1;
-                    } else {
-                        V += ts1;
+                    // ---- carries: thread 0 stores them behind the barrier that ends the fill (every lane has read the old ones by then)
+                    uint64_t nV = 0, nD1 = 0;
+                    if (tid == 0) {
+                        nV = S.nd_v;
+                        nD1 = S.nd_d1;
+                        if (delta2) {
+                            nV += ts2 + (uint64_t)tc * nD1;
+                            nD1 += ts1;
+                        } else {
+                            nV += ts1;
+                        }
                     }
                     N += tc;
                     cnt += tot;
@@ -855,10 +867,14 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
                         if (N != nvar) bail = true;
                     }
                     __syncthreads();
+                    if (tid == 0) {
+                        S.nd_v = nV;
+                        S.nd_d1 = nD1;
+                    }
                     if ((S.flags | S.flags_emit) & 1u) bail = true;
                     if (stream_done && !bail) {
                         const uint32_t last_al = (uint32_t)(vhi - 1);  // aligned position of the last stream byte
-                        if (A[last_al] >= 0x80) bail = true;
+                        if (SE.A[last_al] >= 0x80) bail = true;
                     }
                 }
             } else if (!is_stream && gen_rows < n) {
@@ -866,9 +882,9 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
                 const uint32_t take = min(n - gen_rows, (uint32_t)FU_CAP - cnt);
                 for (uint32_t k = tid; k < take; k += FU_THREADS) {
                     const uint32_t r = gen_rows + k;
-                    const int64_t v = (int64_t)((uint64_t)first_value + (uint64_t)r * (uint64_t)dconst);
-                    RV[base + cnt + k] = dec.conv(v);
-                    if (stale_matters && v == VMB_V_STALE_NAN) S.flags = 1u;
+                    const int64_t v = (int64_t)((uint64_t)SE.first_value + (uint64_t)r * (uint64_t)SE.dconst);
+                    RV[base + cnt + k] = fu_dec(SE).conv(v);
+                    if (SE.stale_matters && v == VMB_V_STALE_NAN) S.flags = 1u;
                 }
                 progressed = take > 0;
                 gen_rows += take;
@@ -882,7 +898,7 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
             if (p >= P.npoints) continue;  // only validating the rest of the stream
 
             // ================= removeCounterResets over the new rows [cnt_old, cnt)  (rollup.go:921)
-            if (do_rcr && cnt > cnt_old) {
+            if (SE.do_rcr && cnt > cnt_old) {
                 const uint32_t nev = S.nev;
                 const double raw_last = RV[base + cnt - 1];
                 if (nev > FU_MAX_EVENTS) {
@@ -957,6 +973,10 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
             }
 
             // ================= points whose window lies inside the resident rows
+            const int32_t start_r = SE.start_r, step32 = SE.step32, win32 = SE.win32, mpi32 = SE.mpi32;
+            const bool lin = SE.lin != 0;
+            const int32_t lin_k = SE.lin_k, iq0 = SE.iq0, jq0 = SE.jq0;
+            const float inv_row = 1.0f / (float)dt_row;
             uint32_t p_end;
             if (all_rows) p_end = P.npoints;
             else {
@@ -969,11 +989,17 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
                 continue;
             }
             {
+                // rate(): the divisor of a full window, its reciprocal (used only when a point's divisor is exactly this one)
+                const int32_t rate_dt = SE.rate_dt, rate_rows = SE.rate_rows;
+                const double rate_D = SE.rate_D, rate_R = SE.rate_R;
+                // a previous sample right in front of the window always passes `ts > tStart - maxPrevInterval` when maxPrevInterval >= dt
+                const bool prev_always = mpi32 >= dt_row;
                 const uint32_t spc = (uint32_t)rc.samples_scanned_per_call;
                 uint32_t sc32 = 0;
+                unsigned long long scanned = 0;
                 const FuVals WV{S.val, base};  // WV[k] = resident row base + k
                 const bool to_aggr = P.aggr_values != nullptr;
-                double* out_row = P.out + (to_aggr ? (size_t)blockIdx.x : (size_t)s) * P.npoints;
+                double* out_row = P.out + (to_aggr ? (size_t)blockIdx.x : (size_t)SE.s) * P.npoints;
                 asm volatile("" : "+l"(out_row));  // (kept in registers: the loops below are tight)
                 auto put = [&](uint32_t q, double v) { out_row[q] = v; };
                 uint32_t sc_interior = spc ? spc : (uint32_t)rate_rows;  // samplesScanned of an interior rate() point
@@ -1046,10 +1072,10 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
                         }
                         put(q, fixed ? (prev_ok ? 0.0 : D_NAN) : qv);
                     } else {
-                        put(q, fu_point<F>(rc, window, max_prev, S.val, n, i, j, q, t_org, dts, scanned));
+                        put(q, fu_point<F>(rc, SE.window, SE.max_prev, S.val, n, i, j, q, SE.t_org, SE.dts, scanned));
                     }
                 }
-                scanned += sc32;
+                S.s_ser[tid] += scanned + sc32;
             }
             p = p_end;
             __syncthreads();
@@ -1067,25 +1093,25 @@ __global__ void __launch_bounds__(FU_THREADS, 4) k_fused_rollup(FusedParams P) {
         }
         // a copy still in flight must land before the buffer is reused by the next series
         if (copy_pending) {
-            mbar_wait(&S.mbar[buf], buf ? par1 : par0);
-            if (buf) par1 ^= 1u; else par0 ^= 1u;
+            mbar_wait(&S.mbar[buf], (par >> buf) & 1u);
+            par ^= 1u << buf;
         }
         if (bail) {
             if (tid == 0) {
                 const unsigned int e = atomicAdd(P.bail_count, 1u);
-                P.bail_list[e] = s;
+                P.bail_list[e] = SE.s;
             }
         } else {
-            scanned_cta += scanned;
+            S.s_thr[tid] += S.s_ser[tid];
             if (P.aggr_values) {  // the finished row -> the group's partial state
                 __syncthreads();
                 const double* row = P.out + (size_t)blockIdx.x * P.npoints;
-                const size_t cell0 = (size_t)P.group_ids[s] * P.npoints;
+                const size_t cell0 = (size_t)P.group_ids[SE.s] * P.npoints;
                 for (uint32_t q = tid; q < P.npoints; q += FU_THREADS) fu_fold(P.aggr_id, P.aggr_values, P.aggr_counts, cell0 + q, row[q]);
             }
         }
     }
-    unsigned long long scanned = scanned_cta;
+    unsigned long long scanned = S.s_thr[tid];
     // block reduce -> one atomic per CTA
     __syncthreads();
 #pragma unroll
