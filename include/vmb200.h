@@ -373,6 +373,21 @@ int vmb_matrix_merge_rows(vmb_ctx* ctx, const double* d_a, const int64_t* a_rows
  * size: groups of more than 2048 series return VMB_ERR_CAP. */
 int vmb_aggr_quantile(vmb_ctx* ctx, const double* d_vals, size_t nseries, size_t points, const uint32_t* group_ids, uint32_t ngroups,
                       const double* phis, double* d_out);
+/* aggr(q) by (...) for any argument q (aggrFuncExt aggr.go:110 with aggrFuncSum :185 ... aggrFuncZScore :493): the non-incremental
+ * aggregates on a DEVICE matrix d_vals[nseries x P].  Not the ids of vmb_aggr_func: those are the incremental callbacks, whose sum
+ * starts from the first value instead of 0 +.  group_ids: HOST, dense ids < ngroups.  Within a group the rows are folded in
+ * ascending row order.  Rows without a non-NaN value belong to no group (removeEmptySeries :124), and a group left with one row
+ * takes the reference's fast path: sum / avg / min / max / geomean return that row as it is, stddev / stdvar 0 where it has a value.
+ *   d_out: [ngroups x P]; rows of groups without a non-empty row are NaN.  SHARE / ZSCORE: [nseries x P] instead, every row
+ *   rewritten from its group's statistics; d_out may be d_vals.
+ *   row_nonempty: HOST, nseries bytes, 1 where the row holds a non-NaN value (as in vmb_topk_apply); the host derives from it which
+ *   groups exist, `limit N` (the first N groups in order of their first non-empty row) and which rows share / zscore return.
+ * Bit-exact except geomean over two or more values (pow).  VMB_ERR_INVALID_ARG for an unknown func, ngroups == 0, a group id >=
+ * ngroups or nseries / points > 2^31 - 1, with d_out untouched.  nseries == 0: d_out is NaN. */
+enum vmb_matrix_aggr { VMB_MA_SUM = 0, VMB_MA_SUM2, VMB_MA_MIN, VMB_MA_MAX, VMB_MA_AVG, VMB_MA_COUNT, VMB_MA_GROUP,
+                       VMB_MA_GEOMEAN, VMB_MA_STDDEV, VMB_MA_STDVAR, VMB_MA_SHARE, VMB_MA_ZSCORE };
+int vmb_aggr_matrix(vmb_ctx* ctx, int func, const double* d_vals, size_t nseries, size_t points, const uint32_t* group_ids,
+                    uint32_t ngroups, double* d_out, unsigned char* row_nonempty);
 
 /* ---- multi-GPU: one process per GPU, the ONE exchange step of the path inside the library (SURVEY 8e) ------------------
  * aggr(rollup(m[d])) by (...): every rank folds its shard of the series into {values, counts}[G x P] (the per-worker

@@ -1766,6 +1766,7 @@ extern "C" int vmb_eval_rollup_aggr_device(vmb_ctx* ctx, const vmb_blocks* b, in
 #include "topk.inc"
 #include "comm.inc"
 #include "matrix_ops.inc"
+#include "aggr_matrix.inc"
 #include "transform.inc"
 
 // ------------------------------------------------------------------------------------------------ batched host encoder

@@ -541,6 +541,30 @@ def transform(name, dev_ptr, nrows, points, *scalar_args, ctx=None):
     check(lib().vmb_transform(ctx.h, TRANSFORM_FUNCS[name], C.c_void_p(int(dev_ptr)), int(nrows), int(points), fp(a1), fp(a2)))
 
 
+MATRIX_AGGR_FUNCS = {n: i for i, n in enumerate(
+    ["sum", "sum2", "min", "max", "avg", "count", "group", "geomean", "stddev", "stdvar", "share", "zscore"])}
+
+
+def aggr_matrix(name, vals_dev_ptr, nseries, points, out_dev_ptr, group_ids=None, ngroups=1, limit=0, ctx=None):
+    """aggr(q) by (...) [limit N] (aggrFuncExt aggr.go:110) on a DEVICE matrix [nseries x points] for any argument q: sum, sum2, min,
+    max, avg, count, group, geomean, stddev, stdvar -> out_dev_ptr [ngroups x points]; share, zscore -> out_dev_ptr [nseries x points]
+    (may be vals_dev_ptr).  Returns the ids of the groups the reference outputs (those with a non-empty row), in order of their first
+    non-empty row and cut at `limit` (0 = no limit); for share / zscore the np.bool_[nseries] mask of the rows it returns instead."""
+    ctx = ctx or _lib.default_context()
+    g = np.zeros(nseries, dtype=np.uint32) if group_ids is None else np.ascontiguousarray(group_ids, dtype=np.uint32)
+    flags = np.zeros(max(nseries, 1), dtype=np.uint8)
+    check(lib().vmb_aggr_matrix(ctx.h, MATRIX_AGGR_FUNCS[name.lower()], C.c_void_p(int(vals_dev_ptr)), int(nseries), int(points),
+                                g.ctypes.data_as(_lib.u32p), int(ngroups), C.c_void_p(int(out_dev_ptr)), flags.ctypes.data_as(_lib.u8p)))
+    nonempty = flags[:nseries].astype(bool)
+    _, first = np.unique(g[nonempty], return_index=True)  # aggrPrepareSeries aggr.go:139: groups in order of first non-empty row
+    groups = g[nonempty][np.sort(first)]
+    if limit > 0:
+        groups = groups[:limit]
+    if name.lower() in ("share", "zscore"):
+        return nonempty & np.isin(g, groups)
+    return groups
+
+
 def aggr_quantile(phis, vals_dev_ptr, nseries, points, out_dev_ptr, group_ids=None, ngroups=1, ctx=None):
     """quantile(phi, q) by (...) / median (phi = 0.5)  aggr.go:1217 on a DEVICE matrix -> out_dev_ptr [ngroups x points]"""
     ctx = ctx or _lib.default_context()
