@@ -904,7 +904,7 @@ __global__ void k_meta_from_offsets(SeriesMeta* meta, const uint64_t* offsets, u
     SeriesMeta m;
     m.start = offsets[s];
     m.n = (uint32_t)(offsets[s + 1] - offsets[s]);
-    m._pad = 3;  // host-built batch: staleness markers / value drops unknown => dropStaleNaNs and removeCounterResets scan
+    m.flags = VMB_SER_STALE | VMB_SER_DROP;  // host-built batch: staleness markers / value drops unknown => dropStaleNaNs and removeCounterResets scan
     m.max_prev_interval = 0;
     m.window = 0;
     meta[s] = m;
@@ -976,7 +976,7 @@ __global__ void __launch_bounds__(128) k_series_from_matrix(const double* __rest
             SeriesMeta mm;
             mm.start = o0;
             mm.n = o;
-            mm._pad = 2u;  // no staleness markers can be left (they are NaNs); value drops unknown => removeCounterResets scans
+            mm.flags = VMB_SER_DROP;  // no staleness markers can be left (they are NaNs); value drops unknown => removeCounterResets scans
             mm.max_prev_interval = 0;
             mm.window = 0;
             meta[s] = mm;

@@ -54,13 +54,37 @@ struct HufJob {
 };
 static_assert(sizeof(HufJob) == 312, "HufJob layout");
 
+// SeriesMeta::flags, bits 0-3; bits 8-23 hold the first row with a value drop (SeriesMeta::first_drop)
+enum : uint32_t {
+    VMB_SER_STALE = 1u,    // the series may hold Prometheus staleness markers: dropStaleNaNs has something to do
+    VMB_SER_DROP = 2u,     // the series may hold a value below its predecessor (or a NaN): removeCounterResets has something to do
+    VMB_SER_MERGED = 4u,   // the series is assembled by k_series_merge
+    VMB_SER_TS_AP = 8u,    // the timestamps are an arithmetic progression (one block, MarshalTypeDeltaConst timestamps, no
+                           // deduplication): the rollup kernel derives them from the row index instead of reading them
+};
+
 struct SeriesMeta {
     uint64_t start;          // first row of the series inside the dense columns
     uint32_t n;              // rows (after trimming / stale-NaN drop)
-    uint32_t _pad;
+    uint32_t flags;          // VMB_SER_* | first_drop() << 8
     int64_t max_prev_interval;
     int64_t window;          // effective window (rollup.go:747-756)
+    // the row removeCounterResets may start from: nothing before the first value drop changes (0: unknown)
+    __host__ __device__ __forceinline__ uint32_t first_drop() const { return (flags >> 8) & 0xffffu; }
+    __host__ __device__ __forceinline__ void set_first_drop(uint32_t row) { flags = (flags & ~(0xffffu << 8)) | ((row & 0xffffu) << 8); }
 };
+static_assert(sizeof(SeriesMeta) == 32, "SeriesMeta layout");
+
+// blk_hi, the per-block word k_decode_columns writes beside blk_lo (the first kept row) for k_series_assemble / k_series_merge:
+// bits 0-14 end of the kept rows (<= 16384), bits 15-28 first row with a value drop, bit 30 "may change under
+// removeCounterResets", bit 31 "holds a staleness marker"
+__host__ __device__ __forceinline__ uint32_t blk_hi_pack(uint32_t end, uint32_t first_drop, bool may_change, bool stale) {
+    return end | (first_drop << 15) | ((uint32_t)may_change << 30) | ((uint32_t)stale << 31);
+}
+__host__ __device__ __forceinline__ uint32_t blk_hi_end(uint32_t w) { return w & 0x7fffu; }
+__host__ __device__ __forceinline__ uint32_t blk_hi_first_drop(uint32_t w) { return (w >> 15) & 0x3fffu; }
+__host__ __device__ __forceinline__ bool blk_hi_may_change(uint32_t w) { return (w >> 30) & 1u; }
+__host__ __device__ __forceinline__ bool blk_hi_stale(uint32_t w) { return w >> 31; }
 
 // ---- small device helpers ---------------------------------------------------------------------------------------
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }

@@ -301,15 +301,15 @@ __global__ void __launch_bounds__(128) k_decode_columns(DecodeParams P) {
             const bool as_int = (P.flags & VMB_DECODE_VALUES_AS_INT64) != 0;
             ve.init(as_int ? (void*)((int64_t*)P.val_out + ro) : (void*)((double*)P.val_out + ro), d.scale, as_int);
             rc = decode_column(src, len, d.val_mt, d.first_value, d.rows, ve, sm);
-            // blk_hi: bits 0-14 end of the kept rows (<= 16384), bits 15-28 first row with a value drop, bit 30 "may change
-            // under removeCounterResets", bit 31 "holds a staleness marker"
-            if (__any_sync(VMB_FULL, ve.saw_stale)) hi |= 0x80000000u;
-            if (__any_sync(VMB_FULL, ve.saw_stale || ve.saw_drop)) {
-                uint32_t fd = ve.first_drop;
+            const bool may_change = __any_sync(VMB_FULL, ve.saw_stale || ve.saw_drop);
+            uint32_t fd = 0;
+            if (may_change) {
+                fd = ve.first_drop;
 #pragma unroll
                 for (int off = 16; off; off >>= 1) fd = min(fd, __shfl_xor_sync(VMB_FULL, fd, off));
-                hi |= 0x40000000u | ((fd < 16384u ? fd : 0u) << 15);
+                fd = fd < 16384u ? fd : 0u;
             }
+            hi = blk_hi_pack(hi, fd, may_change, __any_sync(VMB_FULL, ve.saw_stale));
         }
         if (lane == 0) {
             P.status[b] = rc;

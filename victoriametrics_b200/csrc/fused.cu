@@ -183,7 +183,7 @@ __device__ __forceinline__ void fu_sts_i64(uint32_t val_s, uint32_t row, long lo
 struct FuVals {  // read view for the rollup functions: element i is row r + i
     const double* s;
     uint32_t r;
-    __device__ __forceinline__ double operator[](uint32_t i) const { return fu_ld(s, r + i); }
+    __device__ __forceinline__ double operator[](int32_t i) const { return fu_ld(s, r + i); }
     __device__ __forceinline__ FuVals operator+(uint32_t k) const { return FuVals{s, r + k}; }
     __device__ __forceinline__ FuVals& operator++() { r++; return *this; }
     __device__ __forceinline__ FuVals operator++(int) { FuVals o = *this; r++; return o; }
@@ -194,7 +194,7 @@ struct FuValsRW {  // read/write by absolute row
 };
 struct FuTs {  // timestamps of a MarshalTypeDeltaConst column are never stored: element i is t + i * dt
     int64_t t, dt;
-    __device__ __forceinline__ int64_t operator[](uint32_t i) const { return t + (int64_t)i * dt; }
+    __device__ __forceinline__ int64_t operator[](int64_t i) const { return t + i * dt; }  // (i = -1: the row in front)
     __device__ __forceinline__ FuTs operator+(uint32_t k) const { return FuTs{t + (int64_t)k * dt, dt}; }
     __device__ __forceinline__ FuTs& operator++() { t += dt; return *this; }
     __device__ __forceinline__ FuTs operator++(int) { FuTs o = *this; t += dt; return o; }
@@ -259,75 +259,6 @@ __device__ __forceinline__ void fu_fold(int aggr, double* values, double* counts
     }
 }
 
-// getScrapeInterval (rollup.go:871) + getMaxPrevInterval (:899) + the window rules (:719-756) for a series whose rows sit at
-// t0 + row * dt: same float operations as k_series_prepare on twenty equal intervals
-__device__ void fu_prev_interval_window(const vmb_rollup_cfg& rc, uint32_t n, int64_t dt, int64_t* max_prev_out, int64_t* window_out) {
-    int64_t maxPrev = rc.step;
-    if (rc.start < rc.end) {
-        int64_t si = rc.step;
-        if (n >= 2) {
-            uint32_t k = n - 1 > 20 ? 20 : n - 1;
-            double iv = (double)dt;
-            double nn = (double)k;
-            double rank = 0.6 * (nn - 1);
-            double weight = rank - floor(rank);
-            double q = __dadd_rn(__dmul_rn(iv, 1 - weight), __dmul_rn(iv, weight));
-            int64_t sq = (int64_t)q;
-            if (sq > 0) si = sq;
-        }
-        if (si <= 2 * 1000) maxPrev = si + 4 * si;
-        else if (si <= 4 * 1000) maxPrev = si + 2 * si;
-        else if (si <= 8 * 1000) maxPrev = si + si;
-        else if (si <= 16 * 1000) maxPrev = si + si / 2;
-        else if (si <= 32 * 1000) maxPrev = si + si / 4;
-        else maxPrev = si + si / 8;
-    }
-    if (rc.lookback_delta > 0 && maxPrev > rc.lookback_delta) maxPrev = rc.lookback_delta;
-    if (rc.min_staleness_ms > 0 && maxPrev < rc.min_staleness_ms) maxPrev = rc.min_staleness_ms;
-    int64_t window = rc.window;
-    if (window <= 0) {
-        window = rc.step;
-        if ((rc.flags & VMB_RC_MAY_ADJUST_WINDOW) && window < maxPrev) window = maxPrev;
-        if ((rc.flags & VMB_RC_IS_DEFAULT_ROLLUP) && rc.lookback_delta > 0 && window > rc.lookback_delta) window = rc.lookback_delta;
-    }
-    *max_prev_out = maxPrev;
-    *window_out = window;
-}
-
-// one output point from the window edges i, j (absolute rows) of a series whose rows sit at t_org + row * dt (rollup.go:769-819);
-// rows [i-1, j] are resident
-template <int F>
-__device__ __forceinline__ double fu_point(const vmb_rollup_cfg& rc, int64_t window, int64_t max_prev, const double* sval, uint32_t n,
-                                           uint32_t i, uint32_t j, uint32_t p, int64_t t_org, int64_t dt, unsigned long long& scanned) {
-    const int64_t tEnd = rc.start + (int64_t)p * rc.step;
-    const int64_t tStart = tEnd - window;
-    if (j < i) j = i;
-    WinT<FuVals, FuTs> r;
-    r.prevValue = D_NAN;
-    r.prevTimestamp = tStart - max_prev;
-    const int64_t t_im1 = t_org + ((int64_t)i - 1) * dt;
-    if (i < n && i > 0 && t_im1 > r.prevTimestamp) {
-        r.prevValue = fu_ld(sval, i - 1);
-        r.prevTimestamp = t_im1;
-    }
-    r.values = FuVals{sval, i};
-    r.timestamps = FuTs{t_im1 + dt, dt};
-    r.n = j - i;
-    r.realPrevValue = D_NAN;
-    if (i > 0) {
-        const int64_t curr = r.n > 0 ? t_im1 + dt : tStart;
-        if (rc.lookback_delta == 0 || (curr - t_im1) < rc.lookback_delta) r.realPrevValue = fu_ld(sval, i - 1);
-    }
-    r.realNextValue = j < n ? fu_ld(sval, j) : D_NAN;
-    r.currTimestamp = tEnd;
-    r.idx = p;
-    r.window = window;
-    r.args = rc.args;
-    r.args2 = rc.args2;
-    scanned += rc.samples_scanned_per_call > 0 ? (unsigned long long)rc.samples_scanned_per_call : (unsigned long long)r.n;
-    return call_func(F >= 0 ? F : rc.func_id, r);
-}
-
 __device__ __forceinline__ int32_t fu_floor_div(int32_t a, int32_t b) {  // b > 0
     int32_t q = a / b;
     return q - ((a % b) < 0 ? 1 : 0);
@@ -356,7 +287,10 @@ __device__ void fu_series_setup(const FusedParams& P, uint32_t s, FuSeries* out)
     bail = bail || t_org < P.tr_min || t_org + (int64_t)(n - 1) * dts > P.tr_max;  // rows trimmed by the time range: un-fused path
     int64_t max_prev = 0, window = 0;
     if (!bail) {
-        fu_prev_interval_window(rc, n, dts, &max_prev, &window);
+        // rows sit at t_org + row * dts (n >= 2): every interval getScrapeInterval looks at is dts
+        const PrevWindow pw = prev_interval_window(rc, scrape_interval(rc.step, n - 1 > 20 ? 20 : n - 1, [&](int) { return (double)dts; }));
+        max_prev = pw.max_prev;
+        window = pw.window;
         const int64_t a0 = rc.start - window - max_prev - t_org, a1 = rc.end - t_org;
         bail = !(a0 > -LIM && a0 < LIM && a1 > -LIM && a1 < LIM && window < LIM && max_prev < LIM && rc.step < LIM);
     }
@@ -1044,35 +978,27 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                     j = j < base ? base : (j > base + cnt ? base + cnt : j);
                     if (j < i) j = i;
                     if (F == VMB_RF_RATE) {
-                        // rollupDerivFast (rollup.go:1954), the selects of rate_point_ap with the division through the cached reciprocal
+                        // rollupDerivFast (rollup.go:1954) with the division through the cached reciprocal
                         sc32 += spc ? spc : j - i;
-                        const uint32_t ri = i - base, rj = j - base, nw = j - i;
-                        const bool have_prev = i > 0 && i < n;
-                        const uint32_t ip = have_prev ? ri - 1 : 0u;
-                        const uint32_t i0 = ri < cnt ? ri : cnt - 1;
-                        const uint32_t il = rj ? rj - 1 : 0u;
-                        const double vp = WV[ip], v0 = WV[i0], vl = WV[il];
-                        const int32_t tp = (int32_t)(base + ip) * dt_row;
-                        const bool prev_ok = have_prev && tp > xj - win32 - mpi32 && !isnan(vp);
-                        const bool fixed = prev_ok ? nw == 0 : nw < 2;
-                        const double a = prev_ok ? vp : v0;
-                        int32_t dtm = (int32_t)(il - (prev_ok ? ip : i0)) * dt_row;
-                        dtm = fixed ? 1000 : dtm;
-                        const double x = vl - a;
+                        const RateEdges<int32_t> e = rate_edges(WV, RowTs32{base, dt_row}, base, n, cnt, i, j, xj - win32 - mpi32);
+                        const double x = e.x;
                         double qv;
                         const uint32_t ex = ((uint32_t)__double2hiint(x) >> 20) & 0x7ffu;
-                        if (dtm == rate_dt && (x == 0.0 || ex - 123u < 1800u)) {
-                            // x / D with D = RN(dtm / 1e3), R = RN(1 / D): q = RN(x R), rem = x - q D (exact), RN(q + rem R) is the correctly
+                        if (e.dt == rate_dt && (x == 0.0 || ex - 123u < 1800u)) {
+                            // x / D with D = RN(dt / 1e3), R = RN(1 / D): q = RN(x R), rem = x - q D (exact), RN(q + rem R) is the correctly
                             // rounded quotient (Markstein's step; |x| in [2^-900, 2^900], D in [1e-3, 2^30/1e3]: no under/overflow anywhere)
                             const double q0 = __dmul_rn(x, rate_R);
                             const double rem = __fma_rn(-q0, rate_D, x);
                             qv = x == 0.0 ? x : __fma_rn(rem, rate_R, q0);
                         } else {
-                            qv = x / ms_to_s((int64_t)dtm);
+                            qv = x / ms_to_s((int64_t)e.dt);
                         }
-                        put(q, fixed ? (prev_ok ? 0.0 : D_NAN) : qv);
+                        put(q, e.result(qv));
                     } else {
-                        put(q, fu_point<F>(rc, SE.window, SE.max_prev, S.val, n, i, j, q, SE.t_org, SE.dts, scanned));
+                        // the window's views start at row i; its timestamp is formed as t(i - 1) + dt, which keeps k_fused_rollup<-1> at 92
+                        // registers (t_org + i * dt costs one more)
+                        const int64_t t_im1 = SE.t_org + ((int64_t)i - 1) * SE.dts;
+                        put(q, window_point<F>(rc, FuVals{S.val, i}, FuTs{t_im1 + SE.dts, SE.dts}, i, n, i, j, q, SE.window, SE.max_prev, scanned));
                     }
                 }
                 S.s_ser[tid] += scanned + sc32;

@@ -154,7 +154,6 @@ struct WinT {
     const double* args;
     const double* args2;
 };
-typedef WinT<const double*, const int64_t*> Win;
 
 template <class VP>
 __device__ double stdvar(VP v, uint32_t n) {  // rollup.go:1808
@@ -839,28 +838,24 @@ __global__ void k_series_assemble(RollupParams P) {
     SeriesMeta m;
     m.start = 0;
     m.n = 0;
-    // bit 0: the series may hold Prometheus staleness markers; bit 1: the series may hold a value below its predecessor
-    // (or a NaN), i.e. removeCounterResets may have something to do.  Both come from the decode kernel, per block.
-    // bit 2: the series is assembled by k_series_merge.
-    // bit 3: the timestamps are an arithmetic progression (one block, MarshalTypeDeltaConst timestamps, no deduplication):
-    //        the rollup kernel derives them from the row index instead of reading them.
-    m._pad = 0u;
+    m.flags = 0u;
     m.max_prev_interval = 0;
     m.window = 0;
     bool failed = false;
-    for (uint32_t k = 0; k < nb; k++) {
+    for (uint32_t k = 0; k < nb; k++) {  // staleness markers and value drops: known per block from the decode kernel
         if (P.blk_status[fb + k]) failed = true;
-        m._pad |= (P.blk_hi[fb + k] >> 31) | ((P.blk_hi[fb + k] >> 29) & 2u);  // decode.cu ValEmit
+        if (blk_hi_stale(P.blk_hi[fb + k])) m.flags |= VMB_SER_STALE;
+        if (blk_hi_may_change(P.blk_hi[fb + k])) m.flags |= VMB_SER_DROP;
     }
     const uint64_t moff = P.ser_merge_off ? P.ser_merge_off[s] : ~0ull;
     if (!failed && nb) {
         if (moff != ~0ull) {
             m.start = P.rows_total + moff;
-            m._pad |= 4u | 2u;  // (merged rows interleave blocks: always a candidate for removeCounterResets)
+            m.flags |= VMB_SER_MERGED | VMB_SER_DROP;  // (merged rows interleave blocks: always a candidate for removeCounterResets)
         } else {
             uint64_t lo = ~0ull, hi = 0, kept = 0;
             for (uint32_t k = 0; k < nb; k++) {
-                const uint32_t a = P.blk_lo[fb + k], b = P.blk_hi[fb + k] & 0x7fffu;
+                const uint32_t a = P.blk_lo[fb + k], b = blk_hi_end(P.blk_hi[fb + k]);
                 if (b <= a) continue;  // trimmed away completely
                 const uint64_t r = P.row_off[fb + k];
                 lo = r + a < lo ? r + a : lo;
@@ -869,15 +864,15 @@ __global__ void k_series_assemble(RollupParams P) {
             }
             // a value drop across a block boundary (time-disjoint blocks, laid out in time order): compare the decoded values
             // on both sides of every boundary.  Many blocks per series: no search, the series is simply a candidate.
-            if (nb > 1 && !(m._pad & 2u)) {
-                if (nb > 16) m._pad |= 2u;
+            if (nb > 1 && !(m.flags & VMB_SER_DROP)) {
+                if (nb > 16) m.flags |= VMB_SER_DROP;
                 else {
-                    for (uint32_t k = 0; k < nb && !(m._pad & 2u); k++) {
+                    for (uint32_t k = 0; k < nb && !(m.flags & VMB_SER_DROP); k++) {
                         const uint64_t endk = P.row_off[fb + k] + P.descs[fb + k].rows;  // first row of the next block in layout
                         for (uint32_t j = 0; j < nb; j++) {
                             if (j != k && P.row_off[fb + j] == endk && P.descs[fb + j].rows) {
                                 const double a = P.vals[endk - 1], b = P.vals[endk];
-                                if (!(b - a >= 0)) m._pad |= 2u;  // drop or NaN
+                                if (!(b - a >= 0)) m.flags |= VMB_SER_DROP;  // drop or NaN
                             }
                         }
                     }
@@ -892,11 +887,10 @@ __global__ void k_series_assemble(RollupParams P) {
                     m.n = (uint32_t)kept;
                     // (precisionBits < 64 sends the timestamps through EnsureNonDecreasingSequence, which may move the last one)
                     if (nb == 1 && kept >= 2 && P.descs[fb].ts_mt == 2 && P.descs[fb].precision_bits >= 64 && P.dedup_interval <= 0)
-                        m._pad |= 8u;
-                    if (nb == 1 && P.dedup_interval <= 0 && !(m._pad & 1u)) {
-                        // bits 8-23: the row removeCounterResets may start from (nothing before the first value drop changes)
-                        const uint32_t fd = (P.blk_hi[fb] >> 15) & 0x3fffu, a = P.blk_lo[fb];
-                        if (fd > a) m._pad |= (fd - a) << 8;
+                        m.flags |= VMB_SER_TS_AP;
+                    if (nb == 1 && P.dedup_interval <= 0 && !(m.flags & VMB_SER_STALE)) {
+                        const uint32_t fd = blk_hi_first_drop(P.blk_hi[fb]), a = P.blk_lo[fb];
+                        if (fd > a) m.set_first_drop(fd - a);
                     }
                 }
             }
@@ -946,7 +940,7 @@ __global__ void __launch_bounds__(128) k_series_merge(RollupParams P) {
     for (uint32_t s = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); s < P.nseries; s += warps_per_grid) {
         if (P.ser_merge_off[s] == ~0ull) continue;
         SeriesMeta m = P.meta[s];
-        if (!(m._pad & 4u)) continue;  // failed series
+        if (!(m.flags & VMB_SER_MERGED)) continue;  // failed series
         const uint32_t fb = P.ser_first_block[s], nb = P.ser_nblocks[s];
         MergeHeap H;
         H.h = P.merge_heap + fb;
@@ -956,7 +950,7 @@ __global__ void __launch_bounds__(128) k_series_merge(RollupParams P) {
         H.lane = lane;
         uint32_t hn = 0;
         for (uint32_t k = 0; k < nb; k++) {  // empty blocks never enter the heap (netstorage.go:568)
-            const uint32_t b = fb + k, lo = P.blk_lo[b], hi = P.blk_hi[b] & 0x7fffu;
+            const uint32_t b = fb + k, lo = P.blk_lo[b], hi = blk_hi_end(P.blk_hi[b]);
             if (hi > lo) {
                 if (lane == 0) { H.h[hn] = b; H.next[b] = lo; }
                 hn++;
@@ -967,7 +961,7 @@ __global__ void __launch_bounds__(128) k_series_merge(RollupParams P) {
         uint64_t o = m.start;
         while (hn) {
             const uint32_t top = H.h[0];
-            const uint32_t idx = H.next[top], end = P.blk_hi[top] & 0x7fffu;
+            const uint32_t idx = H.next[top], end = blk_hi_end(P.blk_hi[top]);
             const uint64_t trow = P.row_off[top];
             uint32_t adv, ncopy;
             if (hn == 1) {
@@ -979,7 +973,7 @@ __global__ void __launch_bounds__(128) k_series_merge(RollupParams P) {
                 uint32_t eq = 0;
                 if (P.dedup_interval > 0) {  // equalSamplesPrefix netstorage.go:622: timestamps first, then value bits
                     const uint64_t nrow = P.row_off[nx] + H.next[nx];
-                    const uint32_t lim = min(end - idx, (P.blk_hi[nx] & 0x7fffu) - H.next[nx]);
+                    const uint32_t lim = min(end - idx, blk_hi_end(P.blk_hi[nx]) - H.next[nx]);
                     uint32_t nt = 0;
                     for (; nt < lim; nt += 32) {
                         const uint32_t k = nt + lane;
@@ -1198,6 +1192,46 @@ __device__ __forceinline__ void rcr_chunk(RcrState& st, VP v, uint32_t cb, uint3
     if (max_stale > 0) st.prev_ts = (int64_t)shfl_u64((uint64_t)tt, 31);
 }
 
+// getScrapeInterval (rollup.go:871) from the k >= 1 intervals it looks at: their 0.6 quantile, `step` when that is not
+// positive.  iv(x) is the x-th smallest of the intervals.
+template <class IV>
+__device__ __forceinline__ int64_t scrape_interval(int64_t step, uint32_t k, IV iv) {
+    const double nn = (double)k;
+    const double rank = 0.6 * (nn - 1);
+    const double lower = fmax(0.0, floor(rank));
+    const double upper = fmin(nn - 1, lower + 1);
+    const double weight = rank - floor(rank);
+    const double q = __dadd_rn(__dmul_rn(iv((int)lower), 1 - weight), __dmul_rn(iv((int)upper), weight));
+    const int64_t sq = (int64_t)q;
+    return sq > 0 ? sq : step;
+}
+
+// maxPrevInterval and the effective window of a series whose scrape interval is si: getMaxPrevInterval (rollup.go:899), the
+// lookback / min-staleness clamps and the default-window rules (rollup.go:719-756).  A query of one point ignores si.
+struct PrevWindow {
+    int64_t max_prev, window;
+};
+__device__ __forceinline__ PrevWindow prev_interval_window(const vmb_rollup_cfg& rc, int64_t si) {
+    int64_t maxPrev = rc.step;
+    if (rc.start < rc.end) {
+        if (si <= 2 * 1000) maxPrev = si + 4 * si;
+        else if (si <= 4 * 1000) maxPrev = si + 2 * si;
+        else if (si <= 8 * 1000) maxPrev = si + si;
+        else if (si <= 16 * 1000) maxPrev = si + si / 2;
+        else if (si <= 32 * 1000) maxPrev = si + si / 4;
+        else maxPrev = si + si / 8;
+    }
+    if (rc.lookback_delta > 0 && maxPrev > rc.lookback_delta) maxPrev = rc.lookback_delta;
+    if (rc.min_staleness_ms > 0 && maxPrev < rc.min_staleness_ms) maxPrev = rc.min_staleness_ms;
+    int64_t window = rc.window;
+    if (window <= 0) {
+        window = rc.step;
+        if ((rc.flags & VMB_RC_MAY_ADJUST_WINDOW) && window < maxPrev) window = maxPrev;
+        if ((rc.flags & VMB_RC_IS_DEFAULT_ROLLUP) && rc.lookback_delta > 0 && window > rc.lookback_delta) window = rc.lookback_delta;
+    }
+    return PrevWindow{maxPrev, window};
+}
+
 // one warp per series
 __global__ void __launch_bounds__(128) k_series_prepare(RollupParams P) {
     const int lane = lane_id();
@@ -1209,7 +1243,7 @@ __global__ void __launch_bounds__(128) k_series_prepare(RollupParams P) {
         int64_t* t = P.ts + m.start;
         uint32_t n = m.n;
         // ---- dropStaleNaNs eval.go:1985
-        if ((rc.flags & VMB_RC_DROP_STALE_NANS) && n && (m._pad & 1u)) {  // decoded batches know whether a marker exists
+        if ((rc.flags & VMB_RC_DROP_STALE_NANS) && n && (m.flags & VMB_SER_STALE)) {  // decoded batches know whether a marker exists
             bool has = false;
             for (uint32_t i = lane; i < n; i += 32) has |= is_stale_nan(v[i]);
             if (__any_sync(VMB_FULL, has)) {
@@ -1228,7 +1262,10 @@ __global__ void __launch_bounds__(128) k_series_prepare(RollupParams P) {
                     o += __popc(bal);
                     __syncwarp();
                 }
-                if (o != n) m._pad &= 0xffu & ~8u;  // rows were removed: no arithmetic progression, no known first drop
+                if (o != n) {  // rows were removed: no arithmetic progression, no known first drop
+                    m.flags &= ~VMB_SER_TS_AP;
+                    m.set_first_drop(0);
+                }
                 n = o;
             }
         }
@@ -1240,10 +1277,10 @@ __global__ void __launch_bounds__(128) k_series_prepare(RollupParams P) {
         // first value drop of a series are not touched: the pass starts at the 128-row group that holds it, in the state the
         // sequential loop has there (no correction yet, outputs == inputs).
         const int64_t max_stale = rc.lookback_delta != 0 ? rc.lookback_delta + rc.window : 0;  // rollup.go:380-387
-        if ((rc.flags & VMB_RC_REMOVE_COUNTER_RESETS) && n && (m._pad & 2u)) {
+        if ((rc.flags & VMB_RC_REMOVE_COUNTER_RESETS) && n && (m.flags & VMB_SER_DROP)) {
             RcrState st;
             st.corr = 0.0; st.prev_raw = 0.0; st.prev_out = 0.0; st.prev_ts = 0;
-            const uint32_t r0 = (m._pad >> 8) & 0xffffu;
+            const uint32_t r0 = m.first_drop();
             const uint32_t base0 = r0 >= n ? 0u : (r0 & ~127u);
             if (base0) {
                 st.prev_raw = st.prev_out = v[base0 - 1];
@@ -1332,58 +1369,33 @@ __global__ void __launch_bounds__(128) k_series_prepare(RollupParams P) {
         }
         // ---- maxPrevInterval / window  rollup.go:719-756
         if (lane == 0) {
-            int64_t maxPrev = rc.step;
-            if (rc.start < rc.end) {
-                // getScrapeInterval rollup.go:871: 0.6 quantile of the last <= 20 intervals
-                int64_t si = rc.step;
-                if (n >= 2) {
-                    double iv[20];
-                    uint32_t m2 = n - 1;
-                    uint32_t from = m2 > 20 ? m2 - 20 : 0;
-                    uint32_t k = 0;
-                    int64_t tsPrev = t[n - 1];
-                    for (int i = (int)m2 - 1; i >= (int)from; i--) {
-                        iv[k++] = (double)(tsPrev - t[i]);
-                        tsPrev = t[i];
-                    }
-                    for (uint32_t a = 1; a < k; a++) {  // insertion sort
-                        double x = iv[a];
-                        int b = (int)a - 1;
-                        while (b >= 0 && iv[b] > x) {
-                            iv[b + 1] = iv[b];
-                            b--;
-                        }
-                        iv[b + 1] = x;
-                    }
-                    double nn = (double)k;
-                    double rank = 0.6 * (nn - 1);
-                    double lower = fmax(0.0, floor(rank));
-                    double upper = fmin(nn - 1, lower + 1);
-                    double weight = rank - floor(rank);
-                    double q = __dadd_rn(__dmul_rn(iv[(int)lower], 1 - weight), __dmul_rn(iv[(int)upper], weight));
-                    int64_t sq = (int64_t)q;
-                    if (sq > 0) si = sq;
+            int64_t si = rc.step;
+            if (rc.start < rc.end && n >= 2) {  // (a query of one point does not look at the scrape interval)
+                // getScrapeInterval rollup.go:871: the last <= 20 intervals, sorted
+                double iv[20];
+                uint32_t m2 = n - 1;
+                uint32_t from = m2 > 20 ? m2 - 20 : 0;
+                uint32_t k = 0;
+                int64_t tsPrev = t[n - 1];
+                for (int i = (int)m2 - 1; i >= (int)from; i--) {
+                    iv[k++] = (double)(tsPrev - t[i]);
+                    tsPrev = t[i];
                 }
-                // getMaxPrevInterval rollup.go:899
-                if (si <= 2 * 1000) maxPrev = si + 4 * si;
-                else if (si <= 4 * 1000) maxPrev = si + 2 * si;
-                else if (si <= 8 * 1000) maxPrev = si + si;
-                else if (si <= 16 * 1000) maxPrev = si + si / 2;
-                else if (si <= 32 * 1000) maxPrev = si + si / 4;
-                else maxPrev = si + si / 8;
+                for (uint32_t a = 1; a < k; a++) {  // insertion sort
+                    double x = iv[a];
+                    int b = (int)a - 1;
+                    while (b >= 0 && iv[b] > x) {
+                        iv[b + 1] = iv[b];
+                        b--;
+                    }
+                    iv[b + 1] = x;
+                }
+                si = scrape_interval(rc.step, k, [&](int x) { return iv[x]; });
             }
-            if (rc.lookback_delta > 0 && maxPrev > rc.lookback_delta) maxPrev = rc.lookback_delta;
-            if (rc.min_staleness_ms > 0 && maxPrev < rc.min_staleness_ms) maxPrev = rc.min_staleness_ms;
-            int64_t window = rc.window;
-            if (window <= 0) {
-                window = rc.step;
-                if ((rc.flags & VMB_RC_MAY_ADJUST_WINDOW) && window < maxPrev) window = maxPrev;
-                if ((rc.flags & VMB_RC_IS_DEFAULT_ROLLUP) && rc.lookback_delta > 0 && window > rc.lookback_delta)
-                    window = rc.lookback_delta;
-            }
+            const PrevWindow pw = prev_interval_window(rc, si);
             m.n = n;
-            m.max_prev_interval = maxPrev;
-            m.window = window;
+            m.max_prev_interval = pw.max_prev;
+            m.window = pw.window;
             P.meta[s] = m;
         }
         __syncwarp();
@@ -1448,92 +1460,90 @@ __device__ __forceinline__ double ms_to_s(int64_t dt_ms) {
     return __fma_rn(rem, r, q);
 }
 
-// one output point: rollup.go:769-819.  v/t hold the rows [off, ...) of the series (shared-memory window or the whole
-// series with off == 0); rows [i-1, j] must be resident.
-template <int F>
-__device__ __forceinline__ double rollup_point(const vmb_rollup_cfg& rc, const SeriesMeta& m, const double* v, const int64_t* t,
-                                               uint32_t off, uint32_t n, uint32_t i, uint32_t j, uint32_t p,
-                                               unsigned long long& scanned) {
+// one output point, rollup.go:769-819: the rollupFuncArg of point p from its window edges i, j (absolute rows of a series of
+// n rows), and the function applied to it.  v / t reach the rows from `off` on (v[k], t[k] = row off + k); rows [i-1, j] must
+// be reachable.
+template <int F, class VP, class TP>
+__device__ __forceinline__ double window_point(const vmb_rollup_cfg& rc, VP v, TP t, uint32_t off, uint32_t n, uint32_t i, uint32_t j,
+                                               uint32_t p, int64_t window, int64_t max_prev, unsigned long long& scanned) {
     const int64_t tEnd = rc.start + (int64_t)p * rc.step;
-    const int64_t tStart = tEnd - m.window;
+    const int64_t tStart = tEnd - window;
     if (j < i) j = i;
-    const uint32_t ri = i - off, rj = j - off;  // indices into v / t
-    if (F == VMB_RF_RATE) {
-        // rollupDerivFast rollup.go:1954 on the rollupFuncArg doInternal would build (rollup.go:779-784), hand-flattened
-        scanned += rc.samples_scanned_per_call > 0 ? (unsigned long long)rc.samples_scanned_per_call : (unsigned long long)(j - i);
-        double pv = D_NAN;
-        int64_t pt = 0;
-        if (i < n && i > 0) {
-            int64_t tp = t[ri - 1];
-            if (tp > tStart - m.max_prev_interval) {
-                pv = v[ri - 1];
-                pt = tp;
-            }
-        }
-        const uint32_t nw = j - i;
-        if (isnan(pv)) {
-            if (nw < 2) return D_NAN;
-            pv = v[ri];
-            pt = t[ri];
-        } else if (nw == 0) {
-            return 0.0;
-        }
-        return (v[rj - 1] - pv) / ms_to_s(t[rj - 1] - pt);
-    }
-    Win r;
-    r.prevValue = D_NAN;
-    r.prevTimestamp = tStart - m.max_prev_interval;
-    if (i < n && i > 0 && t[ri - 1] > r.prevTimestamp) {
-        r.prevValue = v[ri - 1];
-        r.prevTimestamp = t[ri - 1];
-    }
-    r.values = v + ri;
-    r.timestamps = t + ri;
+    WinT<VP, TP> r;
+    r.values = v + (i - off);  // the window; [-1] is the row in front of it
+    r.timestamps = t + (i - off);
     r.n = j - i;
+    r.prevValue = D_NAN;
+    r.prevTimestamp = tStart - max_prev;
     r.realPrevValue = D_NAN;
     if (i > 0) {
-        int64_t curr = r.n > 0 ? t[ri] : tStart;
-        if (rc.lookback_delta == 0 || (curr - t[ri - 1]) < rc.lookback_delta) r.realPrevValue = v[ri - 1];
+        const int64_t tp = r.timestamps[-1];
+        const double vp = r.values[-1];
+        if (i < n && tp > r.prevTimestamp) {
+            r.prevValue = vp;
+            r.prevTimestamp = tp;
+        }
+        const int64_t curr = r.n > 0 ? r.timestamps[0] : tStart;
+        if (rc.lookback_delta == 0 || (curr - tp) < rc.lookback_delta) r.realPrevValue = vp;
     }
-    r.realNextValue = j < n ? v[rj] : D_NAN;
+    r.realNextValue = j < n ? r.values[r.n] : D_NAN;
     r.currTimestamp = tEnd;
     r.idx = p;
-    r.window = m.window;
+    r.window = window;
     r.args = rc.args;
     r.args2 = rc.args2;
     scanned += rc.samples_scanned_per_call > 0 ? (unsigned long long)rc.samples_scanned_per_call : (unsigned long long)r.n;
     return call_func(F >= 0 ? F : rc.func_id, r);
 }
 
-// Streaming rollup: one CTA walks one series front to back.  Rows are pulled into shared memory once, in order, with
-// coalesced loads (no per-tile searches in global memory); the CTA computes every output point whose window lies inside the
-// resident rows (threads stride over the points of the fill), then slides the resident range forward keeping only
-// the rows the next point still needs.  Both the samples and the output grid are time-ordered, so this visits each row once.
-//
-// Window seeks: when the window is a multiple of the step (rate(m[5m]) at step 15 s: 20 steps), the left edge of point p is
-// the right edge of point p - window/step, so a fill computes ONE seek per grid time (s_seek[]) instead of two per point.
-//
-// A window that does not fit ROLLUP_CAP rows (huge windows / very dense series) is handled for that tile by reading global
-// memory directly.  F >= 0 instantiates the kernel for one rollup function (the switch in call_func folds away).
-// rate() for one point of a series whose timestamps are t_org + row * dt (rows absolute): same selects as rate_point32 below
-// with the timestamps derived from the row indices
-template <class VP>
-__device__ __forceinline__ double rate_point_ap(uint32_t i, uint32_t j, uint32_t base, uint32_t n, uint32_t cnt, int32_t tsp,
-                                                int32_t dt_row, VP val) {
-    const uint32_t ri = i - base, rj = j - base, nw = j - i;
+// rollupDerivFast (rollup.go:1954) of one point from its window edges i <= j (absolute rows of a series of n rows) with selects
+// instead of branches, up to the division, which each caller does its own way: result(x / (dt / 1e3)).  v / t reach the rows
+// [off, off + cnt) (v[k], t[k] = row off + k), rows [i-1, j) among them; tsp = tStart - maxPrevInterval on the scale of t.
+template <class T>
+struct RateEdges {
+    double x;  // numerator: the last value of the window - the previous sample's value (or the window's first)
+    T dt;      // divisor in ms (1000 where the quotient is not used)
+    bool prev_ok, fixed;
+    __device__ __forceinline__ double result(double q) const { return fixed ? (prev_ok ? 0.0 : D_NAN) : q; }
+};
+template <class VP, class TP, class T>
+__device__ __forceinline__ RateEdges<T> rate_edges(VP v, TP t, uint32_t off, uint32_t n, uint32_t cnt, uint32_t i, uint32_t j, T tsp) {
+    const uint32_t ri = i - off, rj = j - off, nw = j - i;
     const bool have_prev = i > 0 && i < n;
     const uint32_t ip = have_prev ? ri - 1 : 0u;
-    const uint32_t i0 = ri < cnt ? ri : cnt - 1;
     const uint32_t il = rj ? rj - 1 : 0u;
-    const double vp = val[ip], v0 = val[i0], vl = val[il];
-    const int32_t tp = (int32_t)(base + ip) * dt_row;
-    const bool prev_ok = have_prev && tp > tsp && !isnan(vp);
-    const bool fixed = prev_ok ? nw == 0 : nw < 2;
-    const double a = prev_ok ? vp : v0;
-    int32_t dt = (int32_t)(il - (prev_ok ? ip : i0)) * dt_row;
-    dt = fixed ? 1000 : dt;
-    const double qv = (vl - a) / ms_to_s((int64_t)dt);
-    return fixed ? (prev_ok ? 0.0 : D_NAN) : qv;
+    const uint32_t i0 = ri < cnt ? ri : il;  // (ri == cnt only for an empty window, whose first row is not used)
+    const T tp = t[ip], t0 = t[i0], tl = t[il];
+    const double vp = v[ip], v0 = v[i0], vl = v[il];
+    RateEdges<T> e;
+    e.prev_ok = have_prev && tp > tsp && !isnan(vp);
+    e.fixed = e.prev_ok ? nw == 0 : nw < 2;  // no division: 0 with a previous sample, NaN without
+    e.x = vl - (e.prev_ok ? vp : v0);
+    e.dt = e.fixed ? (T)1000 : tl - (e.prev_ok ? tp : t0);
+    return e;
+}
+
+// timestamps relative to the first row of a series whose row r sits at r * dt: element k is row base + k
+struct RowTs32 {
+    uint32_t base;
+    int32_t dt;
+    __device__ __forceinline__ int32_t operator[](uint32_t k) const { return (int32_t)(base + k) * dt; }
+};
+
+// one output point of k_rollup: v / t hold the rows [off, off + cnt) of the series (shared-memory window, or the whole series
+// with off == 0 and cnt == n); rows [i-1, j] must be resident
+template <int F>
+__device__ __forceinline__ double rollup_point(const vmb_rollup_cfg& rc, const SeriesMeta& m, const double* v, const int64_t* t,
+                                               uint32_t off, uint32_t n, uint32_t cnt, uint32_t i, uint32_t j, uint32_t p,
+                                               unsigned long long& scanned) {
+    if (F == VMB_RF_RATE) {
+        if (j < i) j = i;
+        scanned += rc.samples_scanned_per_call > 0 ? (unsigned long long)rc.samples_scanned_per_call : (unsigned long long)(j - i);
+        const RateEdges<int64_t> e =
+            rate_edges(v, t, off, n, cnt, i, j, rc.start + (int64_t)p * rc.step - m.window - m.max_prev_interval);
+        return e.result(e.x / ms_to_s(e.dt));
+    }
+    return window_point<F>(rc, v, t, off, n, i, j, p, m.window, m.max_prev_interval, scanned);
 }
 
 // rows with timestamp <= t_org + xr when row k sits at t_org + k * dt: exact floor division from a float estimate
@@ -1570,25 +1580,16 @@ __device__ __forceinline__ uint32_t seek32(uint32_t n, int32_t xr, float inv_dt,
     return res;
 }
 
-// rollupDerivFast (rollup.go:1954) for one point from the window edges i, j (absolute rows); tsp = tStart - maxPrevInterval
-// as an offset from the first row of the series.  Selects instead of branches; same operations as the generic path.
-__device__ __forceinline__ double rate_point32(uint32_t i, uint32_t j, uint32_t base, uint32_t n, uint32_t cnt, int32_t tsp) {
-    const uint32_t ri = i - base, rj = j - base, nw = j - i;
-    const bool have_prev = i > 0 && i < n;
-    const uint32_t ip = have_prev ? ri - 1 : 0u;
-    const uint32_t i0 = ri < cnt ? ri : cnt - 1;
-    const uint32_t il = rj ? rj - 1 : 0u;
-    const int32_t tp = rs_rt[ip], t0 = rs_rt[i0], tl = rs_rt[il];
-    const double vp = rs_val[ip], v0 = rs_val[i0], vl = rs_val[il];
-    const bool prev_ok = have_prev && tp > tsp && !isnan(vp);
-    const bool fixed = prev_ok ? nw == 0 : nw < 2;  // no division: 0 with a previous sample, NaN without
-    const double a = prev_ok ? vp : v0;
-    int32_t dt = tl - (prev_ok ? tp : t0);
-    dt = fixed ? 1000 : dt;
-    const double qv = (vl - a) / ms_to_s((int64_t)dt);
-    return fixed ? (prev_ok ? 0.0 : D_NAN) : qv;
-}
-
+// Streaming rollup: one CTA walks one series front to back.  Rows are pulled into shared memory once, in order, with
+// coalesced loads (no per-tile searches in global memory); the CTA computes every output point whose window lies inside the
+// resident rows (threads stride over the points of the fill), then slides the resident range forward keeping only
+// the rows the next point still needs.  Both the samples and the output grid are time-ordered, so this visits each row once.
+//
+// Window seeks: when the window is a multiple of the step (rate(m[5m]) at step 15 s: 20 steps), the left edge of point p is
+// the right edge of point p - window/step, so a fill computes ONE seek per grid time (s_seek[]) instead of two per point.
+//
+// A window that does not fit ROLLUP_CAP rows (huge windows / very dense series) is handled for that tile by reading global
+// memory directly.  F >= 0 instantiates the kernel for one rollup function (the switch in call_func folds away).
 template <int F>
 __global__ void __launch_bounds__(ROLLUP_THREADS, 4) k_rollup(RollupParams P) {
     const vmb_rollup_cfg& rc = P.cfg;
@@ -1633,7 +1634,7 @@ __global__ void __launch_bounds__(ROLLUP_THREADS, 4) k_rollup(RollupParams P) {
         int32_t dt_row = 0;
         float inv_row = 0.0f;
         bool ap = false;
-        if (fast && (m._pad & 8u) && n >= 2) {
+        if (fast && (m.flags & VMB_SER_TS_AP) && n >= 2) {
             const int64_t d = tg[1] - tg[0];
             if (d > 0 && d < ((int64_t)1 << 30) && (int64_t)(n - 1) * d < ((int64_t)1 << 30)) {
                 ap = true;
@@ -1681,7 +1682,7 @@ __global__ void __launch_bounds__(ROLLUP_THREADS, 4) k_rollup(RollupParams P) {
                     int64_t tEnd = rc.start + (int64_t)q * rc.step;
                     uint32_t i = upper_bound_ts(tg, n, tEnd - m.window);
                     uint32_t j = upper_bound_ts(tg, n, tEnd);
-                    out[q] = rollup_point<F>(rc, m, vg, tg, 0u, n, i, j, q, scanned);
+                    out[q] = rollup_point<F>(rc, m, vg, tg, 0u, n, n, i, j, q, scanned);
                 }
                 p = p_end;
                 if (p < P.npoints) {  // restart the resident range at the first row the next point needs
@@ -1707,46 +1708,36 @@ __global__ void __launch_bounds__(ROLLUP_THREADS, 4) k_rollup(RollupParams P) {
             if (p_end - p > ROLLUP_SEEKS - wsteps_cap) p_end = p + (ROLLUP_SEEKS - wsteps_cap);
             const uint32_t np = p_end - p;
             const int64_t t_first = (cnt && !ap) ? rs_ts[0] : 0, t_last = (cnt && !ap) ? rs_ts[cnt - 1] : 0;
-            if (ap) {
-                // edges from the row arithmetic (absolute rows, clamped to the resident range), then the points
+            if (fast) {
+                // branch-free 32-bit edges, then the rate() points.  Edges and timestamps come from the row arithmetic in
+                // arithmetic-progression mode (edges clamped to the resident range), else from the resident rs_rt.
                 const int32_t x0r = start_r + ((int32_t)p - (int32_t)wsteps) * step32;
-#pragma unroll 2
-                for (uint32_t q = tid; q < np + wsteps; q += ROLLUP_THREADS) {
-                    uint32_t e = seek_ap(x0r + (int32_t)q * step32, dt_row, inv_row, n);
-                    e = e < base ? base : (e > base + cnt ? base + cnt : e);
-                    rs_seek[q] = (unsigned short)(e - base);
-                }
-                __syncthreads();
-                const int32_t ts0 = start_r + (int32_t)p * step32 - win32 - mpi32;
-                const uint32_t spc = (uint32_t)rc.samples_scanned_per_call;
-                uint32_t sc32 = 0;
-#pragma unroll 2
-                for (uint32_t q = tid; q < np; q += ROLLUP_THREADS) {
-                    const uint32_t i = base + rs_seek[q];
-                    const uint32_t j = max(i, base + rs_seek[q + wsteps]);
-                    sc32 += spc ? spc : j - i;
-                    out[p + q] = rate_point_ap(i, j, base, n, cnt, ts0 + (int32_t)q * step32, dt_row, rs_val);
-                }
-                scanned += sc32;
-            } else if (fast) {
-                // branch-free 32-bit edges and rate() points (same arithmetic as rollup_point<VMB_RF_RATE>)
-                const int32_t r_first = rs_rt[0], r_last = rs_rt[cnt - 1];
-                const int32_t x0r = start_r + ((int32_t)p - (int32_t)wsteps) * step32;
-#pragma unroll 2
-                for (uint32_t q = tid; q < np + wsteps; q += ROLLUP_THREADS)
-                    rs_seek[q] = (unsigned short)seek32(cnt, x0r + (int32_t)q * step32, inv_dt, r_first, r_last, t_org);
-                __syncthreads();
                 const int32_t ts0 = start_r + (int32_t)p * step32 - win32 - mpi32;  // tStart - maxPrevInterval of point p
                 const uint32_t spc = (uint32_t)rc.samples_scanned_per_call;
-                uint32_t sc32 = 0;
+                auto rate_fill = [&](auto seek, auto ts) {
 #pragma unroll 2
-                for (uint32_t q = tid; q < np; q += ROLLUP_THREADS) {
-                    const uint32_t i = base + rs_seek[q];
-                    const uint32_t j = max(i, base + rs_seek[q + wsteps]);
-                    sc32 += spc ? spc : j - i;
-                    out[p + q] = rate_point32(i, j, base, n, cnt, ts0 + (int32_t)q * step32);
+                    for (uint32_t q = tid; q < np + wsteps; q += ROLLUP_THREADS) rs_seek[q] = (unsigned short)seek(x0r + (int32_t)q * step32);
+                    __syncthreads();
+                    uint32_t sc32 = 0;
+#pragma unroll 2
+                    for (uint32_t q = tid; q < np; q += ROLLUP_THREADS) {
+                        const uint32_t i = base + rs_seek[q];
+                        const uint32_t j = max(i, base + rs_seek[q + wsteps]);
+                        sc32 += spc ? spc : j - i;
+                        const RateEdges<int32_t> e = rate_edges(rs_val, ts, base, n, cnt, i, j, ts0 + (int32_t)q * step32);
+                        out[p + q] = e.result(e.x / ms_to_s((int64_t)e.dt));
+                    }
+                    scanned += sc32;
+                };
+                if (ap) {
+                    rate_fill([&](int32_t x) {
+                        const uint32_t e = seek_ap(x, dt_row, inv_row, n);
+                        return (e < base ? base : (e > base + cnt ? base + cnt : e)) - base;
+                    }, RowTs32{base, dt_row});
+                } else {
+                    const int32_t r_first = rs_rt[0], r_last = rs_rt[cnt - 1];
+                    rate_fill([&](int32_t x) { return seek32(cnt, x, inv_dt, r_first, r_last, t_org); }, (const int32_t*)rs_rt);
                 }
-                scanned += sc32;
             } else if (shared_seeks) {
                 const int64_t x0 = rc.start + ((int64_t)p - (int64_t)wsteps) * rc.step;
 #pragma unroll 2
@@ -1755,14 +1746,14 @@ __global__ void __launch_bounds__(ROLLUP_THREADS, 4) k_rollup(RollupParams P) {
                 __syncthreads();
 #pragma unroll 2
                 for (uint32_t q = tid; q < np; q += ROLLUP_THREADS)
-                    out[p + q] = rollup_point<F>(rc, m, rs_val, rs_ts, base, n, base + rs_seek[q], base + rs_seek[q + wsteps], p + q, scanned);
+                    out[p + q] = rollup_point<F>(rc, m, rs_val, rs_ts, base, n, cnt, base + rs_seek[q], base + rs_seek[q + wsteps], p + q, scanned);
             } else {
                 for (uint32_t q = tid; q < np; q += ROLLUP_THREADS) {
                     const int64_t tEnd = rc.start + (int64_t)(p + q) * rc.step;
                     const uint32_t i = base + seek_resident(rs_ts, cnt, tEnd - m.window, inv_dt, t_first, t_last);
                     const uint32_t j = base + seek_resident(rs_ts, cnt, tEnd, inv_dt, t_first, t_last);
                     // rows before `base` are not resident: the slide rule below keeps row i-1 of the first point resident
-                    out[p + q] = rollup_point<F>(rc, m, rs_val, rs_ts, base, n, i, j, p + q, scanned);
+                    out[p + q] = rollup_point<F>(rc, m, rs_val, rs_ts, base, n, cnt, i, j, p + q, scanned);
                 }
             }
             p = p_end;
