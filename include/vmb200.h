@@ -388,6 +388,22 @@ enum vmb_matrix_aggr { VMB_MA_SUM = 0, VMB_MA_SUM2, VMB_MA_MIN, VMB_MA_MAX, VMB_
                        VMB_MA_GEOMEAN, VMB_MA_STDDEV, VMB_MA_STDVAR, VMB_MA_SHARE, VMB_MA_ZSCORE };
 int vmb_aggr_matrix(vmb_ctx* ctx, int func, const double* d_vals, size_t nseries, size_t points, const uint32_t* group_ids,
                     uint32_t ngroups, double* d_out, unsigned char* row_nonempty);
+/* The order-statistic aggregates by (...) for any argument q, on a DEVICE matrix d_vals[nseries x P], with no cap on the group size:
+ * quantiles (aggrFuncQuantiles aggr.go:1162), mad (:942), mode (:446), distinct (:423), outliers_iqr (:952), outliers_mad (:1004).
+ * Each reads the sorted non-NaN values of every (group, point) cell.  group_ids, row_nonempty and the groups without a non-empty
+ * row as in vmb_aggr_matrix; none of the six has a one-row fast path.  args: HOST.
+ *   QUANTILES     args = nargs >= 1 phis; d_out [nargs x ngroups x P], phi-major (one [ngroups x P] matrix per phi)
+ *   MAD, MODE, DISTINCT  nargs == 0; d_out [ngroups x P]
+ *   OUTLIERS_IQR  nargs == 0; OUTLIERS_MAD: args = nargs == P tolerances, one per point.  d_out is not used (may be NULL);
+ *                 row_selected: HOST, nseries bytes, 1 for a row with a point outside its cell's bounds.
+ * Bit-exact except the sign of a zero quantiles / mode result where a tied rank holds both -0.0 and +0.0 (the reference's sort is
+ * not stable there either).  VMB_ERR_INVALID_ARG for an unknown func, ngroups == 0, a group id >= ngroups, a wrong nargs, a missing
+ * pointer or nseries / points > 2^31 - 1, with the outputs untouched; VMB_ERR_NOMEM when the scratch (at most 2 GiB of keys, or two
+ * point columns of them if one column needs more) cannot be had.  nseries == 0: d_out is NaN. */
+enum vmb_order_aggr { VMB_OA_QUANTILES = 0, VMB_OA_MAD, VMB_OA_MODE, VMB_OA_DISTINCT, VMB_OA_OUTLIERS_IQR, VMB_OA_OUTLIERS_MAD };
+int vmb_aggr_order(vmb_ctx* ctx, int func, const double* d_vals, size_t nseries, size_t points, const uint32_t* group_ids,
+                   uint32_t ngroups, const double* args, size_t nargs, double* d_out, unsigned char* row_nonempty,
+                   unsigned char* row_selected);
 
 /* ---- multi-GPU: one process per GPU, the ONE exchange step of the path inside the library (SURVEY 8e) ------------------
  * aggr(rollup(m[d])) by (...): every rank folds its shard of the series into {values, counts}[G x P] (the per-worker

@@ -80,6 +80,7 @@ struct vmb_ctx {
     DevBuf bail, sub_arrays;  // fused path: series handed to the un-fused pipeline, and that sub-batch's arrays
     DevBuf enc_vals, enc_deltas, enc_out, enc_meta;  // vmb_marshal_columns_gpu
     DevBuf aggr_state, grp_ids;  // vmb_eval_rollup_aggr_dist: {values, counts}[G x P]; device copy of the per-series group ids
+    DevBuf oa_keys, oa_keys2, oa_cell, oa_meta;  // vmb_aggr_order: a point batch's keys, its merge buffer, per-cell bounds, sort plan
     void* comm = nullptr;     // ncclComm_t (comm.inc); nullptr = single GPU
     bool comm_owned = false;
     int comm_ranks = 1, comm_rank = 0;
@@ -178,7 +179,8 @@ extern "C" void vmb_ctx_destroy(vmb_ctx* c) {
     if (c->col_cache) vmb_series_free(c->col_cache);
     c->col_cache = nullptr;
     DevBuf* bufs[] = {&c->zscratch, &c->zlit, &c->zstatus, &c->zjobs, &c->zws, &c->args1, &c->args2, &c->rolled,
-                      &c->counters, &c->tmp_out, &c->grp, &c->mheap, &c->mnext, &c->zseq, &c->bail, &c->sub_arrays, &c->aggr_state, &c->grp_ids, &c->enc_vals, &c->enc_deltas, &c->enc_out, &c->enc_meta};
+                      &c->counters, &c->tmp_out, &c->grp, &c->mheap, &c->mnext, &c->zseq, &c->bail, &c->sub_arrays, &c->aggr_state, &c->grp_ids, &c->enc_vals, &c->enc_deltas, &c->enc_out, &c->enc_meta,
+                      &c->oa_keys, &c->oa_keys2, &c->oa_cell, &c->oa_meta};
     for (DevBuf* b : bufs) b->release();
     for (cudaEvent_t e : c->ev)
         if (e) cudaEventDestroy(e);
@@ -1767,6 +1769,7 @@ extern "C" int vmb_eval_rollup_aggr_device(vmb_ctx* ctx, const vmb_blocks* b, in
 #include "comm.inc"
 #include "matrix_ops.inc"
 #include "aggr_matrix.inc"
+#include "aggr_order.inc"
 #include "transform.inc"
 
 // ------------------------------------------------------------------------------------------------ batched host encoder

@@ -565,6 +565,40 @@ def aggr_matrix(name, vals_dev_ptr, nseries, points, out_dev_ptr, group_ids=None
     return groups
 
 
+ORDER_AGGR_FUNCS = {n: i for i, n in enumerate(["quantiles", "mad", "mode", "distinct", "outliers_iqr", "outliers_mad"])}
+
+
+def aggr_order(name, vals_dev_ptr, nseries, points, out_dev_ptr=None, group_ids=None, ngroups=1, phis=None, tolerance=None, limit=0,
+               ctx=None):
+    """The order-statistic aggregates by (...) [limit N] (aggrFuncExt aggr.go:110) on a DEVICE matrix [nseries x points], any group
+    size: quantiles(phis) -> out_dev_ptr [len(phis) x ngroups x points] (phi-major); mad, mode, distinct -> out_dev_ptr [ngroups x
+    points]; outliers_iqr, outliers_mad(tolerance) write no matrix.  phis and tolerance: a number or an array (tolerance: one per
+    point).  Returns the ids of the groups the reference outputs, in order of their first non-empty row and cut at `limit` (0 = no
+    limit); for outliers_iqr / outliers_mad the np.bool_[nseries] mask of the rows it returns instead."""
+    ctx = ctx or _lib.default_context()
+    name = name.lower()
+    g = np.zeros(nseries, dtype=np.uint32) if group_ids is None else np.ascontiguousarray(group_ids, dtype=np.uint32)
+    args = None
+    if name == "quantiles":
+        args = np.ascontiguousarray(np.asarray(phis, dtype=np.float64).reshape(-1))
+    elif name == "outliers_mad":
+        args = np.ascontiguousarray(np.broadcast_to(np.asarray(tolerance, dtype=np.float64), (points,)))
+    nonempty = np.zeros(max(nseries, 1), dtype=np.uint8)
+    selected = np.zeros(max(nseries, 1), dtype=np.uint8)
+    check(lib().vmb_aggr_order(ctx.h, ORDER_AGGR_FUNCS[name], C.c_void_p(int(vals_dev_ptr)), int(nseries), int(points),
+                               g.ctypes.data_as(_lib.u32p), int(ngroups), args.ctypes.data_as(_lib.f64p) if args is not None else None,
+                               0 if args is None else args.size, C.c_void_p(int(out_dev_ptr or 0)), nonempty.ctypes.data_as(_lib.u8p),
+                               selected.ctypes.data_as(_lib.u8p)))
+    ne = nonempty[:nseries].astype(bool)
+    _, first = np.unique(g[ne], return_index=True)  # aggrPrepareSeries aggr.go:139: groups in order of first non-empty row
+    groups = g[ne][np.sort(first)]
+    if limit > 0:
+        groups = groups[:limit]
+    if name in ("outliers_iqr", "outliers_mad"):
+        return selected[:nseries].astype(bool) & np.isin(g, groups)
+    return groups
+
+
 def aggr_quantile(phis, vals_dev_ptr, nseries, points, out_dev_ptr, group_ids=None, ngroups=1, ctx=None):
     """quantile(phi, q) by (...) / median (phi = 0.5)  aggr.go:1217 on a DEVICE matrix -> out_dev_ptr [ngroups x points]"""
     ctx = ctx or _lib.default_context()
