@@ -67,6 +67,9 @@ int vmb_ctx_set_fused(vmb_ctx* ctx, int enable);
 /* CTAs of the fused kernel's (persistent) grid on the current device for rate(): a series list of at most this many series runs
  * one series per CTA.  Never more than 132 x 5. */
 int vmb_fused_grid(void);
+/* The same for rate() when the call runs its fused series in chunks, the zstd stage of the next chunk beside the fused kernel
+ * (at most 132 x 4 CTAs: the rest of the SM is left to the zstd kernels; the other functions keep vmb_fused_grid()). */
+int vmb_fused_grid_chunked(void);
 int vmb_ctx_synchronize(vmb_ctx* ctx);
 const char* vmb_last_error(void);
 int vmb_version(void);

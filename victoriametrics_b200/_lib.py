@@ -78,6 +78,7 @@ def lib():
         "vmb_last_error": (C.c_char_p, []),
         "vmb_version": (C.c_int, []),
         "vmb_fused_grid": (C.c_int, []),
+        "vmb_fused_grid_chunked": (C.c_int, []),
         "vmb_ctx_launch_count": (C.c_uint64, [vp]),
         "vmb_block_desc_from_header": (C.c_int, [C.POINTER(BlockDesc), u8p, u8p]),
         "vmb_block_header_marshal": (C.c_int, [u8p, C.POINTER(BlockDesc), u8p]),

@@ -67,6 +67,9 @@ struct DevBuf {  // grow-only device buffer
 // ev[ST_FUSED] where the aggregate ends, so stage s spans ev[s] .. ev[s + 1]; eval_fused says which events it records.
 enum Stage { ST_ZSTD, ST_DECODE, ST_PREAMBLE, ST_ROLLUP, ST_AGGR, ST_FUSED, ST__COUNT };
 
+#define FUSED_CHUNKS_DEFAULT 4u /* eval_fused: chunks of the fused series list (VMB_FUSED_CHUNKS overrides) */
+#define FUSED_CHUNKS_MAX 64u
+
 struct vmb_ctx {
     int device = 0;
     cudaStream_t stream = 0;
@@ -85,6 +88,13 @@ struct vmb_ctx {
     bool comm_owned = false;
     int comm_ranks = 1, comm_rank = 0;
     bool fused = true;           // vmb_ctx_set_fused: series that qualify go through the fused decode+rollup kernel (fused.cu)
+    // fused path: the series are cut into this many chunks; the zstd stage of chunk k + 1 runs on zstream beside the fused
+    // kernel of chunk k (1 = zstd of the whole batch, then one fused launch)
+    uint32_t fused_chunks = 0;  // 0: eval_fused's own choice (fused_chunks()); VMB_FUSED_CHUNKS sets it
+    // CTAs per SM of the fused grid (<= FU_CTAS_PER_SM); 0 = FU_CTAS_PER_SM_OVERLAP when chunked, FU_CTAS_PER_SM otherwise
+    uint32_t fused_ctas_per_sm = 0;
+    cudaStream_t zstream = nullptr;               // created on first use, non-blocking
+    std::vector<cudaEvent_t> zev;                 // zev[k]: the zstd stage of chunk k is done
     int64_t dedup_interval = 0;  // storage.SetDedupInterval (lib/storage/dedup.go:15), ms; 0 = deduplication off
     struct vmb_series* col_cache = nullptr;  // decoded columns of the one-call device paths, sized for the largest batch seen
     void* h_pinned = nullptr;  // small pinned staging area for counters
@@ -116,6 +126,9 @@ struct vmb_blocks {
     // values MarshalType), the others, and host copies of what a sub-batch for the un-fused pipeline is built from
     uint32_t* d_fused_list = nullptr;
     std::vector<uint32_t> h_fused, h_unfused, h_ser_first, h_ser_nblocks;
+    // d_huf_list holds the columns no fused series reads first, then the values columns of h_fused in that order:
+    // h_huf_upto[j] = where the entries of h_fused[j..] begin (size h_fused.size() + 1)
+    std::vector<uint32_t> h_huf_upto;
     std::vector<vmb_block_desc> h_descs;
     std::vector<ColInfo> h_cols;
 };
@@ -163,7 +176,15 @@ extern "C" int vmb_ctx_create(int device, vmb_ctx** out) {
     }
     vmb_ctx* c = new vmb_ctx();
     c->device = device;
-    c->fused = getenv("VMB_NO_FUSED") == nullptr;  // A/B switch for profiles
+    c->fused = getenv("VMB_NO_FUSED") == nullptr;  // A/B switches for profiles
+    if (const char* s = getenv("VMB_FUSED_CHUNKS")) {
+        const long v = atol(s);
+        c->fused_chunks = v < 1 ? 1u : (v > (long)FUSED_CHUNKS_MAX ? FUSED_CHUNKS_MAX : (uint32_t)v);
+    }
+    if (const char* s = getenv("VMB_FUSED_CTAS_PER_SM")) {
+        const long v = atol(s);
+        c->fused_ctas_per_sm = v < 1 ? 1u : (v > FU_CTAS_PER_SM ? (uint32_t)FU_CTAS_PER_SM : (uint32_t)v);
+    }
     for (cudaEvent_t& e : c->ev) CU(cudaEventCreate(&e));
     CU(cudaHostAlloc(&c->h_pinned, 4096, cudaHostAllocDefault));
     *out = c;
@@ -184,6 +205,8 @@ extern "C" void vmb_ctx_destroy(vmb_ctx* c) {
     for (DevBuf* b : bufs) b->release();
     for (cudaEvent_t e : c->ev)
         if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : c->zev) cudaEventDestroy(e);
+    if (c->zstream) cudaStreamDestroy(c->zstream);
     if (c->h_pinned) cudaFreeHost(c->h_pinned);
     if (c->pipe && c->pipe_destroy) c->pipe_destroy(c->pipe);
     delete c;
@@ -382,7 +405,7 @@ extern "C" uint64_t vmb_blocks_compressed_bytes(const vmb_blocks* b) { return b 
 struct BlocksPlan {
     std::vector<ColInfo> cols;
     std::vector<uint64_t> row_off;
-    std::vector<uint32_t> huf, gen, bad, ser_first, ser_nblocks, fused, unfused;
+    std::vector<uint32_t> huf, gen, bad, ser_first, ser_nblocks, fused, unfused, huf_upto;
     std::vector<uint64_t> ser_merge_off;
     uint64_t rows = 0, compressed = 0, scratch_total = 0, merge_rows = 0, seq_total = 0;
     bool needs_lit = false;
@@ -489,6 +512,20 @@ static int plan_blocks(BlocksPlan& pl, const vmb_block_desc* descs, size_t nbloc
                         d.val_mt >= 1 && d.val_mt <= 6 && pl.cols[2 * fb + 1].kind != VMB_ZK_BAD;
         (ok ? pl.fused : pl.unfused).push_back((uint32_t)s);
     }
+    // order the Huffman jobs by the fused series that reads them, so that the zstd stage of any run of consecutive fused
+    // series is one range of the list (eval_fused's chunks); the order of the jobs changes no output
+    std::vector<uint32_t> fpos(2 * nblocks, UINT32_MAX);
+    for (size_t j = 0; j < pl.fused.size(); j++) fpos[2 * (size_t)pl.ser_first[pl.fused[j]] + 1] = (uint32_t)j;
+    std::stable_sort(pl.huf.begin(), pl.huf.end(), [&](uint32_t a, uint32_t b) {
+        return fpos[a] + 1u < fpos[b] + 1u;  // UINT32_MAX (read by no fused series) wraps to 0: first
+    });
+    pl.huf_upto.assign(pl.fused.size() + 1, (uint32_t)pl.huf.size());
+    for (size_t i = pl.huf.size(); i-- > 0;) {
+        const uint32_t j = fpos[pl.huf[i]];
+        if (j == UINT32_MAX) break;
+        pl.huf_upto[j] = (uint32_t)i;
+    }
+    for (size_t j = pl.fused.size(); j-- > 0;) pl.huf_upto[j] = std::min(pl.huf_upto[j], pl.huf_upto[j + 1]);
     return 0;
 }
 
@@ -601,6 +638,7 @@ static int blocks_upload_impl(vmb_ctx* ctx, const vmb_block_desc* descs, size_t 
     b->h_ser_nblocks = pl.ser_nblocks;
     b->h_fused = pl.fused;
     b->h_unfused = pl.unfused;
+    b->h_huf_upto = pl.huf_upto;
     *out = b;
     return VMB_OK;
 }
@@ -669,9 +707,26 @@ __global__ void k_set_status(int32_t* status, const uint32_t* list, uint32_t n, 
     if (i < n) status[list[i]] = v;
 }
 
+// the Huffman-literal frames d_huf_list[h0, h1) of `b` on stream st: headers, literals, sequences (Z as run_zstd set it up)
+static void zstd_huf_range(vmb_ctx* ctx, const vmb_blocks* b, ZstdParams Z, uint32_t h0, uint32_t h1, cudaStream_t st) {
+    if (h0 >= h1) return;
+    Z.jobs = (HufJob*)ctx->zjobs.p + h0;
+    Z.list = b->d_huf_list + h0;
+    Z.count = h1 - h0;
+    launch_zstd_prepare(Z, st);
+    launch_huf_decode(Z, st);
+    count_launch(ctx, 2);
+    if (b->needs_lit) {
+        launch_zstd_sequences(Z, st);
+        count_launch(ctx, 2);
+    }
+}
+
 // zstd stage: every compressed column of `b` is decompressed into ctx->zscratch (at ColInfo::scratch_off); per-column status
-// in ctx->zstatus ([2 * nblocks] int32).  *d_zstatus_out = nullptr when the batch holds no zstd column.
-static int run_zstd(vmb_ctx* ctx, const vmb_blocks* b, int32_t** d_zstatus_out) {
+// in ctx->zstatus ([2 * nblocks] int32).  *d_zstatus_out = nullptr when the batch holds no zstd column.  With huf_end < n_huf
+// only the Huffman frames d_huf_list[0, huf_end) are decoded here and *Zrest receives what zstd_huf_range needs for the others.
+static int run_zstd(vmb_ctx* ctx, const vmb_blocks* b, int32_t** d_zstatus_out, uint32_t huf_end = UINT32_MAX,
+                    ZstdParams* Zrest = nullptr) {
     cudaStream_t st = ctx->stream;
     *d_zstatus_out = nullptr;
     if (b->n_huf + b->n_gen + b->n_bad == 0) return VMB_OK;
@@ -703,19 +758,9 @@ static int run_zstd(vmb_ctx* ctx, const vmb_blocks* b, int32_t** d_zstatus_out) 
         Z.ws = ctx->zws.p;
         Z.ws_count = ws_threads;
     }
-    if (b->n_huf) {
-        if ((rc = ctx->zjobs.reserve((size_t)b->n_huf * sizeof(HufJob)))) return rc;
-        Z.jobs = (HufJob*)ctx->zjobs.p;
-        Z.list = b->d_huf_list;
-        Z.count = b->n_huf;
-        launch_zstd_prepare(Z, st);
-        launch_huf_decode(Z, st);
-        count_launch(ctx, 2);
-        if (b->needs_lit) {
-            launch_zstd_sequences(Z, st);
-            count_launch(ctx, 2);
-        }
-    }
+    if (b->n_huf && (rc = ctx->zjobs.reserve((size_t)b->n_huf * sizeof(HufJob)))) return rc;
+    if (Zrest) *Zrest = Z;
+    zstd_huf_range(ctx, b, Z, 0, std::min(huf_end, b->n_huf), st);
     if (b->n_gen) {
         Z.list = b->d_gen_list;
         Z.count = b->n_gen;
@@ -1500,14 +1545,39 @@ extern "C" int vmb_fused_grid(void) {
     static const uint32_t grid = fused_grid(k_fused_rollup<VMB_RF_RATE>);
     return (int)grid;
 }
+extern "C" int vmb_fused_grid_chunked(void) {
+    return (int)std::min<uint32_t>((uint32_t)vmb_fused_grid(), VMB_SMS * FU_CTAS_PER_SM_OVERLAP);
+}
 
-static void launch_fused(const FusedParams& P, cudaStream_t st) {
+// CTAs per SM of the fused grid of a call cut into C chunks: FU_CTAS_PER_SM, or FU_CTAS_PER_SM_OVERLAP for rate() beside the
+// zstd stage of the next chunk (VMB_FUSED_CTAS_PER_SM overrides both, for measurements)
+// chunks of a fused call: FUSED_CHUNKS_DEFAULT when the zstd stage of chunks 1.. has Huffman frames to hide under the fused
+// kernel, else 1 (nothing to overlap: the 5-CTA one-shot schedule)
+static uint32_t fused_chunks(const vmb_ctx* ctx, const vmb_blocks* b) {
+    const size_t nf = b->h_fused.size();
+    uint32_t C = ctx->fused_chunks ? ctx->fused_chunks : FUSED_CHUNKS_DEFAULT;
+    if (C > nf) C = (uint32_t)nf;
+    if (C <= 1 || b->n_huf == 0) return 1;
+    return b->h_huf_upto[nf / C] < b->n_huf ? C : 1u;
+}
+
+static uint32_t fused_ctas_per_sm(const vmb_ctx* ctx, uint32_t C, const vmb_rollup_cfg* cfg) {
+    if (ctx->fused_ctas_per_sm) return ctx->fused_ctas_per_sm;
+    // rate()'s fused kernel costs about as much as the zstd stage: giving up a fused CTA per SM to the Huffman kernel pays.  The
+    // heavier functions (avg / max / quantile_over_time: 2-3.5x the zstd stage) lose more on the fused side than the overlap gains
+    // and keep 5; their chunks still overlap where fused CTAs leave room (DESIGN.md section 8)
+    return C > 1 && cfg->func_id == VMB_RF_RATE ? FU_CTAS_PER_SM_OVERLAP : FU_CTAS_PER_SM;
+}
+
+// ctas_per_sm (<= FU_CTAS_PER_SM) caps the grid below what the occupancy calculator allows
+static void launch_fused(const FusedParams& P, uint32_t ctas_per_sm, cudaStream_t st) {
     if (!P.nlist) return;
     const size_t smem0 = FUSED_SMEM;
 #define FUSED_LAUNCH(KERNEL, SMEM)                                                                                \
     do {                                                                                                          \
         static const uint32_t grid0 = fused_grid(KERNEL);                                                         \
-        uint32_t grid = grid0 > P.nlist ? P.nlist : grid0;                                                        \
+        uint32_t grid = std::min(grid0, VMB_SMS * ctas_per_sm);                                                   \
+        if (grid > P.nlist) grid = P.nlist;                                                                       \
         KERNEL<<<grid, FU_THREADS, (SMEM), st>>>(P);                                                              \
     } while (0)
     switch (P.cfg.func_id) {  // the value-only functions of BASELINE.json's configs get their own instantiation
@@ -1602,8 +1672,11 @@ __global__ void k_aggr_init(int aggr, double* dv, double* dc, size_t n) {
 
 // decode + preamble + rollup of an uploaded block set through the fused kernel, into d_out or, with af, folded into af's state
 // (initialised here) instead of written to a [series x P] matrix.  Synchronises the stream once (the bail count has to reach the
-// host); the counters are left on the device.  Events: ev[ST_ZSTD] .. ev[ST_DECODE] the zstd stage, ev[ST_DECODE] ..
-// ev[ST_PREAMBLE] the fused kernel, ev[ST_ROLLUP] .. ev[ST_AGGR] the un-fused sub-batch.
+// host); the counters are left on the device.  The fused series run in ctx->fused_chunks chunks: the zstd stage of chunk k + 1
+// runs on ctx->zstream while chunk k's fused kernel runs on the ctx stream, ordered by events only (nothing waits for the two
+// kernels to share an SM).  Events, all on the ctx stream: ev[ST_ZSTD] .. ev[ST_DECODE] the zstd work nothing overlaps (the
+// columns of the un-fused series, the generic frames and chunk 0), ev[ST_DECODE] .. ev[ST_PREAMBLE] first fused launch to last
+// fused completion, ev[ST_ROLLUP] .. ev[ST_AGGR] the un-fused sub-batch.
 static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t tr_max, const vmb_rollup_cfg* cfg, int64_t points,
                       double* d_out, const Counters& c, const AggrTarget* af) {
     cudaStream_t st = ctx->stream;
@@ -1615,24 +1688,17 @@ static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t
         k_aggr_init<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(af->aggr_id, af->d_values, af->d_counts, cells);
         count_launch(ctx);
     }
-    if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_ZSTD], st));
-    int32_t* d_zstatus = nullptr;
-    if ((rc = run_zstd(ctx, b, &d_zstatus))) return rc;
-    if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_DECODE], st));
     const size_t nf = b->h_fused.size();
+    // everything that can fail before any work is forked to zstream
     if ((rc = ctx->bail.reserve((nf + 2) * sizeof(uint32_t)))) return rc;
     unsigned int* d_bail_count = (unsigned int*)ctx->bail.p;
     uint32_t* d_bail_list = (uint32_t*)ctx->bail.p + 2;
-    CU(cudaMemsetAsync(d_bail_count, 0, 8, st));
     FusedParams F;
     memset(&F, 0, sizeof(F));
     if ((rc = upload_cfg_args(ctx, cfg, points, &F.cfg))) return rc;
     F.descs = b->d_descs;
     F.cols = b->d_cols;
     F.payload = b->d_payload;
-    F.scratch = (const uint8_t*)ctx->zscratch.p;
-    F.zstd_status = d_zstatus;
-    F.ser_list = b->d_fused_list;
     F.ser_first_block = b->d_ser_first;
     F.out = d_out;
     if (af) {  // one scratch row per CTA (launch_fused caps the grid at VMB_SMS * FU_CTAS_PER_SM CTAs)
@@ -1646,12 +1712,55 @@ static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t
     F.scanned = c.d_scanned;
     F.bail_list = d_bail_list;
     F.bail_count = d_bail_count;
-    F.nlist = (uint32_t)nf;
     F.npoints = (uint32_t)points;
     F.tr_min = tr_min;
     F.tr_max = tr_max;
-    launch_fused(F, st);
-    count_launch(ctx);
+    // chunk k = the fused series [nf * k / C, nf * (k + 1) / C); its Huffman frames are d_huf_list[huf_upto[..]] of those bounds
+    const uint32_t C = fused_chunks(ctx, b);
+    auto chunk_begin = [&](uint32_t k) { return (uint32_t)(nf * k / C); };
+    if (C > 1) {
+        if (!ctx->zstream) CU(cudaStreamCreateWithFlags(&ctx->zstream, cudaStreamNonBlocking));
+        while (ctx->zev.size() < C) {
+            cudaEvent_t e;
+            CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+            ctx->zev.push_back(e);
+        }
+    }
+    if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_ZSTD], st));
+    int32_t* d_zstatus = nullptr;
+    ZstdParams Z = {};
+    // on st: everything but the Huffman frames of chunks 1..C-1 (= the whole stage when C == 1)
+    if ((rc = run_zstd(ctx, b, &d_zstatus, C > 1 ? b->h_huf_upto[chunk_begin(1)] : UINT32_MAX, &Z))) return rc;
+    if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_DECODE], st));
+    // st joins zstream on every way out of here, errors included, so that the next call cannot reuse the zstd buffers under it
+    struct Join {
+        cudaStream_t st;
+        cudaEvent_t done = nullptr;
+        ~Join() {
+            if (done) cudaStreamWaitEvent(st, done, 0);
+        }
+    } join{st};
+    if (C > 1) {  // the rest on zstream, one chunk after the other, behind what st has queued so far
+        CU(cudaEventRecord(ctx->zev[0], st));
+        CU(cudaStreamWaitEvent(ctx->zstream, ctx->zev[0], 0));
+        for (uint32_t k = 1; k < C; k++) {
+            zstd_huf_range(ctx, b, Z, b->h_huf_upto[chunk_begin(k)], b->h_huf_upto[chunk_begin(k + 1)], ctx->zstream);
+            cudaError_t e = cudaEventRecord(ctx->zev[k], ctx->zstream);
+            if (e == cudaSuccess) join.done = ctx->zev[k];
+            CU(e);
+        }
+    }
+    CU(cudaMemsetAsync(d_bail_count, 0, 8, st));
+    F.scratch = (const uint8_t*)ctx->zscratch.p;
+    F.zstd_status = d_zstatus;
+    const uint32_t ctas_per_sm = fused_ctas_per_sm(ctx, C, cfg);
+    for (uint32_t k = 0; k < C; k++) {  // chunk k starts when its zstd stage is done (chunk 0's ran on st)
+        if (k) CU(cudaStreamWaitEvent(st, ctx->zev[k], 0));
+        F.ser_list = b->d_fused_list + chunk_begin(k);
+        F.nlist = chunk_begin(k + 1) - chunk_begin(k);
+        launch_fused(F, ctas_per_sm, st);
+        count_launch(ctx);
+    }
     if (ctx->timing) CU(cudaEventRecord(ctx->ev[ST_PREAMBLE], st));
     CU(cudaGetLastError());
     unsigned int* h_bail = (unsigned int*)((char*)ctx->h_pinned + PIN_BAIL);

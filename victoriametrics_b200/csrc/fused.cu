@@ -37,6 +37,7 @@
 #define FU_THREADS 128
 #define FU_WARPS 4
 #define FU_CTAS_PER_SM 5                  /* __launch_bounds__ minimum: 5 x ~43 KB of shared memory, 96 registers per thread */
+#define FU_CTAS_PER_SM_OVERLAP 4          /* grid beside the zstd stage of the next chunk: leaves 16 k registers, ~50 KB */
 #define FU_CAP 4096                       /* rows of one series resident in shared memory */
 #define FU_G 2                            /* 16-byte groups per lane and fill: 4 warps x 32 lanes x 32 bytes = one 4 KB fill */
 #define FU_TILE (512 * FU_G)
