@@ -353,7 +353,11 @@ int vmb_group_first_value(vmb_ctx* ctx, const double* d_vals, size_t nseries, si
  * every value, NaN included, like doTransformValues :195; row functions walk each series in point order like the reference (float
  * addition order is part of the result).  arg1 / arg2: HOST arrays of `points` values = getScalar of the scalar arguments:
  *   clamp(q, min, max): arg1 = min, arg2 = max;  clamp_min / clamp_max: arg1;  round(q, nearest): arg1 = nearest, arg2 =
- *   math.Pow10(-e) with (_, e) = decimal.FromFloat(nearest) (transform.go:2341; vmb_float_to_decimal gives e).  Others: NULL.
+ *   math.Pow10(-e) with (_, e) = decimal.FromFloat(nearest) (transform.go:2341; vmb_float_to_decimal gives e).
+ *   smooth_exponential(q, sf): arg1 = sf (getScalar(args[1], 1)).  Others: NULL.
+ * smooth_exponential (:1664): leading NaNs, then leading +-Infs are skipped (if nothing but +-Infs follows, nothing is cut); avg
+ * starts at the first kept value, which stays as it is; later NaNs stay, a later +-Inf becomes the current avg, any other v
+ * becomes avg = avg*(1-sf) + v*sf with sf = arg1 at the point's own index, NaN -> 1, clamped to [0, 1].
  * exp / ln / log2 / log10 / trigonometric / hyperbolic functions are the CUDA math library's (<= 2 ulp from Go's); everything else is
  * bit-exact. */
 enum vmb_transform_func {
@@ -364,9 +368,39 @@ enum vmb_transform_func {
      * keep_last_value / keep_next_value (:1214, :1237), remove_resets = removeCounterResetsMaybeNaNs (:2906) */
     VMB_TF_RUNNING_SUM = 32, VMB_TF_RUNNING_MIN, VMB_TF_RUNNING_MAX, VMB_TF_RUNNING_AVG, VMB_TF_RANGE_SUM, VMB_TF_RANGE_MIN,
     VMB_TF_RANGE_MAX, VMB_TF_RANGE_AVG, VMB_TF_RANGE_FIRST, VMB_TF_RANGE_LAST, VMB_TF_KEEP_LAST_VALUE, VMB_TF_KEEP_NEXT_VALUE,
-    VMB_TF_REMOVE_RESETS, VMB_TF_INTERPOLATE /* :1261 */
+    VMB_TF_REMOVE_RESETS, VMB_TF_INTERPOLATE /* :1261 */, VMB_TF_SMOOTH_EXPONENTIAL /* :1664 */
 };
 int vmb_transform(vmb_ctx* ctx, int func, double* d_matrix, size_t nrows, size_t points, const double* arg1, const double* arg2);
+/* The transforms that reduce a whole series and then rewrite it (app/vmselect/promql/transform.go), in place on a DEVICE matrix
+ * [nrows x points], row by row.  args: HOST, the getScalar(...)[0] of the function's scalar argument as the host has it; the
+ * library applies the reference's own math.Abs(z) and phi /= 2.
+ *   STDDEV, STDVAR (:1550, :1566 -> rollup.go:1803,1808)  nargs 0.  Welford over the row, NaNs skipped; a one-point row is 0 (the
+ *                 len(values) == 1 fast path counts NaNs), a row without a value NaN.  Every point, NaN ones included, gets it.
+ *   ZSCORE (:1408)  nargs 0.  (v - avg) / stddev at every point, avg = mean() (:1425: sum / n over the non-NaN values, 0/0 for
+ *                 none), not Welford's running mean.
+ *   TRIM_ZSCORE (:1379)  nargs 1, args[0] = z.  NaN where |v - avg| / stddev > |z| (a NaN comparison trims nothing).
+ *   NORMALIZE (:1347)  nargs 0.  vMin / vMax over the non-NaN values, d = vMax - vMin; a row where d is +-Inf (one without a value
+ *                 included) is dropped by the reference: left as it is with row_kept[row] = 0.  Kept rows (row_kept 1) get
+ *                 (v - vMin) / d at every point; such a row can be all NaN.  row_kept: HOST, nrows bytes, required here only.
+ *   LINEAR_REGRESSION (:1513 -> rollup.go:1099)  nargs 1, args[0] = step in ms (a positive integer): the points' timestamps are
+ *                 start + j*step and only t - t0 = j*step is read.  areConstValues (rollup.go:1137) on the raw row (any NaN makes
+ *                 it non-constant unless points == 1), sums over the non-NaN values with dt = float64(j*step)/1e3, the 1e-6 tDiff
+ *                 guard; every point gets v + k*float64(j*step)/1e3 in Go's order, without FMA.
+ *   QUANTILE (:1582)  nargs 1, args[0] = phi.  quantileSorted (aggr.go:922) of the sorted non-NaN values goes to the last non-NaN
+ *                 point, then setLastValues (:1650) fills the row with the last non-NaN value it then holds (a NaN result there
+ *                 leaves the one before it, if any); phi < 0, > 1, NaN: -Inf, +Inf, NaN.  A row without a value stays as it is.
+ *   MAD (:1534 -> rollup.go:1476)  nargs 0.  The median, then the median of |v - median| with NaNs dropped, at every point.
+ *   TRIM_OUTLIERS (:1437)  nargs 1, args[0] = k.  NaN where |v - median| > k * mad.
+ *   TRIM_SPIKES (:1465)  nargs 1, args[0] = phi.  phi /= 2; NaN where v > quantileSorted(1 - phi) or v < quantileSorted(phi) of
+ *                 the sorted non-NaN values; NaN points stay, and an empty row or a NaN phi trims nothing.
+ * Bit-exact except the sign of a zero QUANTILE result where a tied rank holds both -0.0 and +0.0 (the reference's sort is not
+ * stable there either).  VMB_ERR_INVALID_ARG for an unknown func, a wrong nargs, a missing args or (NORMALIZE) row_kept, a step
+ * that is not a positive integer (or puts (points - 1) * step past int64), or nrows / points > 2^31 - 1; VMB_ERR_NOMEM when the sort's scratch (at most 2 GiB of keys, or
+ * two rows of them if one row needs more) cannot be had; the matrix is untouched in both cases.  nrows == 0 or points == 0: no-op. */
+enum vmb_range_func { VMB_RS_STDDEV = 0, VMB_RS_STDVAR, VMB_RS_ZSCORE, VMB_RS_TRIM_ZSCORE, VMB_RS_NORMALIZE,
+                      VMB_RS_LINEAR_REGRESSION, VMB_RS_QUANTILE, VMB_RS_MAD, VMB_RS_TRIM_OUTLIERS, VMB_RS_TRIM_SPIKES };
+int vmb_transform_range(vmb_ctx* ctx, int func, double* d_matrix, size_t nrows, size_t points, const double* args, size_t nargs,
+                        unsigned char* row_kept);
 /* mergeSeries rollup_result_cache.go:618: d_dst[nrows x (pa + pb)], row i = d_a[a_rows[i]] ++ d_b[b_rows[i]]; a negative index
  * stands for a series missing on that side (NaNs, :677-690).  a_rows / b_rows: HOST, matched by metric name by the caller. */
 int vmb_matrix_merge_rows(vmb_ctx* ctx, const double* d_a, const int64_t* a_rows, size_t pa, const double* d_b, const int64_t* b_rows,

@@ -83,7 +83,8 @@ struct vmb_ctx {
     DevBuf bail, sub_arrays;  // fused path: series handed to the un-fused pipeline, and that sub-batch's arrays
     DevBuf enc_vals, enc_deltas, enc_out, enc_meta;  // vmb_marshal_columns_gpu
     DevBuf aggr_state, grp_ids;  // vmb_eval_rollup_aggr_dist: {values, counts}[G x P]; device copy of the per-series group ids
-    DevBuf oa_keys, oa_keys2, oa_cell, oa_meta;  // vmb_aggr_order: a point batch's keys, its merge buffer, per-cell bounds, sort plan
+    // vmb_aggr_order / vmb_transform_range: a batch's keys, its merge buffer, per-cell (per-row) statistics, sort plan
+    DevBuf oa_keys, oa_keys2, oa_cell, oa_meta;
     void* comm = nullptr;     // ncclComm_t (comm.inc); nullptr = single GPU
     bool comm_owned = false;
     int comm_ranks = 1, comm_rank = 0;
@@ -1880,6 +1881,7 @@ extern "C" int vmb_eval_rollup_aggr_device(vmb_ctx* ctx, const vmb_blocks* b, in
 #include "aggr_matrix.inc"
 #include "aggr_order.inc"
 #include "transform.inc"
+#include "range_transform.inc"
 
 // ------------------------------------------------------------------------------------------------ batched host encoder
 #include <atomic>

@@ -155,21 +155,30 @@ struct WinT {
     const double* args2;
 };
 
-template <class VP>
-__device__ double stdvar(VP v, uint32_t n) {  // rollup.go:1808
-    if (n == 0) return D_NAN;
-    if (n == 1) return 0;
+// stdvar rollup.go:1808 in step form: add() takes the values in order, result(n) applies the fast paths on n = len(values),
+// NaNs counted.  Shared by the rollup windows and the whole-row range_stddev / range_stdvar / range_zscore (range_transform.inc).
+struct Welford {
     double avg = 0, count = 0, q = 0;
-    for (uint32_t i = 0; i < n; i++) {
-        double x = v[i];
-        if (isnan(x)) continue;
+    __device__ __forceinline__ void add(double x) {
+        if (isnan(x)) return;
         count += 1;
         double avgNew = avg + (x - avg) / count;
         q += (x - avg) * (x - avgNew);
         avg = avgNew;
     }
-    if (count == 0) return D_NAN;
-    return q / count;
+    __device__ __forceinline__ double result(uint64_t n) const {
+        if (n == 0) return D_NAN;
+        if (n == 1) return 0;
+        if (count == 0) return D_NAN;
+        return q / count;
+    }
+};
+template <class VP>
+__device__ double stdvar(VP v, uint32_t n) {
+    Welford w;
+    if (n > 1)
+        for (uint32_t i = 0; i < n; i++) w.add(v[i]);
+    return w.result(n);
 }
 template <class W>
 __device__ double r_sum(const W& r) {
@@ -216,6 +225,32 @@ __device__ double r_scrape_interval(const W& r) {  // rollup.go:2067
     return ((double)(r.timestamps[r.n - 1] - r.prevTimestamp) / 1e3) / (double)r.n;
 }
 
+// linearRegression rollup.go:1108-1134 (after the empty and constant cases) in step form: add() takes the non-NaN (dt, v) pairs
+// in order, fit() gives (v, k).  Shared by the rollup windows and the whole-row range_linear_regression (range_transform.inc).
+struct LinRegSums {
+    double vSum = 0, tSum = 0, tvSum = 0, ttSum = 0;
+    int cnt = 0;
+    __device__ __forceinline__ void add(double dt, double v) {
+        vSum += v;
+        tSum += dt;
+        tvSum = __dadd_rn(tvSum, __dmul_rn(dt, v));  // no FMA contraction: Go does not fuse on amd64
+        ttSum = __dadd_rn(ttSum, __dmul_rn(dt, dt));
+        cnt++;
+    }
+    __device__ __forceinline__ void fit(double* vout, double* kout) const {
+        if (cnt == 0) {
+            *vout = D_NAN;
+            *kout = D_NAN;
+            return;
+        }
+        double k = 0;
+        double tDiff = __dsub_rn(ttSum, __ddiv_rn(__dmul_rn(tSum, tSum), (double)cnt));
+        if (fabs(tDiff) >= 1e-6) k = __ddiv_rn(__dsub_rn(tvSum, __ddiv_rn(__dmul_rn(tSum, vSum), (double)cnt)), tDiff);
+        *vout = __dsub_rn(__ddiv_rn(vSum, (double)cnt), __ddiv_rn(__dmul_rn(k, tSum), (double)cnt));
+        *kout = k;
+    }
+};
+
 template <class W>
 __device__ void linear_regression(const W& r, double* vout, double* kout) {  // rollup.go:1099
     auto values = r.values;
@@ -236,28 +271,13 @@ __device__ void linear_regression(const W& r, double* vout, double* kout) {  // 
         *kout = 0;
         return;
     }
-    double vSum = 0, tSum = 0, tvSum = 0, ttSum = 0;
-    int cnt = 0;
+    LinRegSums s;
     for (uint32_t i = 0; i < n; i++) {
         double v = values[i];
         if (isnan(v)) continue;
-        double dt = (double)(r.timestamps[i] - r.currTimestamp) / 1e3;
-        vSum += v;
-        tSum += dt;
-        tvSum = __dadd_rn(tvSum, __dmul_rn(dt, v));  // no FMA contraction: Go does not fuse on amd64
-        ttSum = __dadd_rn(ttSum, __dmul_rn(dt, dt));
-        cnt++;
+        s.add((double)(r.timestamps[i] - r.currTimestamp) / 1e3, v);
     }
-    if (cnt == 0) {
-        *vout = D_NAN;
-        *kout = D_NAN;
-        return;
-    }
-    double k = 0;
-    double tDiff = __dsub_rn(ttSum, __ddiv_rn(__dmul_rn(tSum, tSum), (double)cnt));
-    if (fabs(tDiff) >= 1e-6) k = __ddiv_rn(__dsub_rn(tvSum, __ddiv_rn(__dmul_rn(tSum, vSum), (double)cnt)), tDiff);
-    *vout = __dsub_rn(__ddiv_rn(vSum, (double)cnt), __ddiv_rn(__dmul_rn(k, tSum), (double)cnt));
-    *kout = k;
+    s.fit(vout, kout);
 }
 
 template <class W>

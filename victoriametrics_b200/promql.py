@@ -502,7 +502,7 @@ TRANSFORM_FUNCS = {n: i for i, n in enumerate(
      "acosh", "atanh", "deg", "rad", "sgn", "clamp", "clamp_min", "clamp_max", "round"])}
 TRANSFORM_FUNCS.update({n: 32 + i for i, n in enumerate(
     ["running_sum", "running_min", "running_max", "running_avg", "range_sum", "range_min", "range_max", "range_avg", "range_first",
-     "range_last", "keep_last_value", "keep_next_value", "remove_resets", "interpolate"])})
+     "range_last", "keep_last_value", "keep_next_value", "remove_resets", "interpolate", "smooth_exponential"])})
 
 
 def _go_pow10(n):
@@ -516,14 +516,15 @@ def _go_pow10(n):
 
 def transform(name, dev_ptr, nrows, points, *scalar_args, ctx=None):
     """transform.go value functions in place on a DEVICE matrix [nrows x points] (vmb_transform).  scalar_args: the function's scalar
-    arguments (numbers or per-point arrays, getScalar): clamp(min, max), clamp_min(min), clamp_max(max), round(nearest = 1)"""
+    arguments (numbers or per-point arrays, getScalar): clamp(min, max), clamp_min(min), clamp_max(max), round(nearest = 1),
+    smooth_exponential(sf)"""
     ctx = ctx or _lib.default_context()
     name = name.lower()
     bc = lambda x: np.ascontiguousarray(np.broadcast_to(np.asarray(x, dtype=np.float64), (points,)))
     a1 = a2 = None
     if name == "clamp":
         a1, a2 = bc(scalar_args[0]), bc(scalar_args[1])
-    elif name in ("clamp_min", "clamp_max"):
+    elif name in ("clamp_min", "clamp_max", "smooth_exponential"):
         a1 = bc(scalar_args[0])
     elif name == "round":
         a1 = bc(scalar_args[0] if scalar_args else 1.0)
@@ -539,6 +540,31 @@ def transform(name, dev_ptr, nrows, points, *scalar_args, ctx=None):
         a2 = np.ascontiguousarray(p10u[inv])
     fp = lambda a: a.ctypes.data_as(_lib.f64p) if a is not None else None
     check(lib().vmb_transform(ctx.h, TRANSFORM_FUNCS[name], C.c_void_p(int(dev_ptr)), int(nrows), int(points), fp(a1), fp(a2)))
+
+
+RANGE_FUNCS = {n: i for i, n in enumerate(
+    ["range_stddev", "range_stdvar", "range_zscore", "range_trim_zscore", "range_normalize", "range_linear_regression",
+     "range_quantile", "range_mad", "range_trim_outliers", "range_trim_spikes"])}
+_RANGE_ONE_ARG = ("range_trim_zscore", "range_quantile", "range_trim_outliers", "range_trim_spikes")
+
+
+def transform_range(name, dev_ptr, nrows, points, *scalar_args, step=None, ctx=None):
+    """transform.go functions that reduce a whole series and rewrite it, in place on a DEVICE matrix [nrows x points]
+    (vmb_transform_range).  scalar_args: range_quantile(phi), range_trim_spikes(phi), range_trim_outliers(k), range_trim_zscore(z),
+    each a number or a per-point array of which the first value counts (getScalar(...)[0]); range_linear_regression needs the
+    query's step in ms.  Returns the np.bool_[nrows] mask of the rows range_normalize keeps, None for the others."""
+    ctx = ctx or _lib.default_context()
+    name = name.lower()
+    args = None
+    if name in _RANGE_ONE_ARG:
+        args = np.ascontiguousarray(np.asarray(scalar_args[0], dtype=np.float64).reshape(-1)[:1])
+    elif name == "range_linear_regression":
+        args = np.array([step], dtype=np.float64)
+    kept = np.zeros(max(int(nrows), 1), dtype=np.uint8) if name == "range_normalize" else None
+    check(lib().vmb_transform_range(ctx.h, RANGE_FUNCS[name], C.c_void_p(int(dev_ptr)), int(nrows), int(points),
+                                    args.ctypes.data_as(_lib.f64p) if args is not None else None, 0 if args is None else args.size,
+                                    kept.ctypes.data_as(_lib.u8p) if kept is not None else None))
+    return kept[:nrows].astype(bool) if kept is not None else None
 
 
 MATRIX_AGGR_FUNCS = {n: i for i, n in enumerate(
