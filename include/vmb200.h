@@ -441,6 +441,35 @@ enum vmb_order_aggr { VMB_OA_QUANTILES = 0, VMB_OA_MAD, VMB_OA_MODE, VMB_OA_DIST
 int vmb_aggr_order(vmb_ctx* ctx, int func, const double* d_vals, size_t nseries, size_t points, const uint32_t* group_ids,
                    uint32_t ngroups, const double* args, size_t nargs, double* d_out, unsigned char* row_nonempty,
                    unsigned char* row_selected);
+/* The histogram functions over Prometheus `le` buckets (app/vmselect/promql/transform.go:634-1169) on a DEVICE matrix d_buckets
+ * [nrows x P], one bucket series per row; read only, it must not overlap an output.  `vmrange` buckets stay with the host.
+ *   group_ids: HOST, one per row, the dense id of the row's label set without `le` (groupLeTimeseries :1097); UINT32_MAX for a row
+ *              without an `le` label or whose `le` does not parse (:1102, :1106): it belongs to no group.
+ *   les:       HOST, one per row, the parsed `le`.
+ *   args:      HOST.  QUANTILE: nargs = nphi x P, a block of P phis (getScalar) per phi: one phi is histogram_quantile, several are
+ *              histogram_quantiles with d_out [nphi x ngroups x P], phi-major.  SHARE: nargs = P, one le per point.  FRACTION:
+ *              nargs = 2P, the lower le of every point, then the upper.  AVG, STDDEV, STDVAR: nargs = 0.
+ *   d_out:     [ngroups x P] (QUANTILE: [nphi x ngroups x P]).
+ *   d_lower, d_upper: both or neither, QUANTILE with one phi and SHARE only: the boundsLabel series [ngroups x P] each
+ *              (:1064-1086, :705-728).
+ *   out_nonempty: HOST, one byte per output row -- the d_out rows, then the d_lower rows, then the d_upper rows --, 1 where the row
+ *              holds a non-NaN value (removeEmptySeries exec.go:133).
+ * Each group's rows are ordered as Go's sort.Slice(xss, xss[i].le < xss[j].le) orders up to 12 elements: a stable insertion sort,
+ * a NaN le left where that loop leaves it; the library uses this order for every group size (for more than 12 rows with equal or
+ * NaN le values Go's pdqsort may order them otherwise).  Per (group, point):
+ *   QUANTILE, SHARE, FRACTION: mergeSameLE (:1151) sums consecutive equal le into the first in order, fixBrokenBuckets (:1122) turns a
+ *     NaN first bucket into 0 and a NaN or smaller later one into the value before it (not for a single bucket), then the loops of
+ *     :1010-1056 (vLast == 0 before the phi < 0 / > 1 checks, lastNonInf falling back to NaN), :661-697 and :759-795.
+ *   AVG, STDDEV, STDVAR (:876-931): the raw rows in that order, +-Inf le skipped, weights v - vPrev, stdvar < 0 clamped to 0, stddev =
+ *     sqrt(stdvar).
+ * Bit-identical to the Go loops.  A group without rows is NaN.  The query errors of the reference (histogram_fraction's lower >= upper
+ * :749) stay with the host.  VMB_ERR_INVALID_ARG for an unknown func, a wrong nargs, bounds on a function without them, a missing
+ * pointer, a group id >= ngroups other than UINT32_MAX, or nrows / points > 2^31 - 1, with the outputs untouched.  nrows == 0,
+ * points == 0 or ngroups == 0: no-op. */
+enum vmb_hist_func { VMB_HF_QUANTILE = 0, VMB_HF_SHARE, VMB_HF_FRACTION, VMB_HF_AVG, VMB_HF_STDDEV, VMB_HF_STDVAR };
+int vmb_histogram(vmb_ctx* ctx, int func, const double* d_buckets, size_t nrows, size_t points, const uint32_t* group_ids,
+                  const double* les, uint32_t ngroups, const double* args, size_t nargs, double* d_out, double* d_lower,
+                  double* d_upper, unsigned char* out_nonempty);
 
 /* ---- multi-GPU: one process per GPU, the ONE exchange step of the path inside the library (SURVEY 8e) ------------------
  * aggr(rollup(m[d])) by (...): every rank folds its shard of the series into {values, counts}[G x P] (the per-worker

@@ -137,6 +137,7 @@ def lib():
         "vmb_aggr_order": (C.c_int, [vp, C.c_int, vp, sz, sz, u32p, C.c_uint32, f64p, sz, vp, u8p, u8p]),
         "vmb_transform": (C.c_int, [vp, C.c_int, vp, sz, sz, f64p, f64p]),
         "vmb_transform_range": (C.c_int, [vp, C.c_int, vp, sz, sz, f64p, sz, u8p]),
+        "vmb_histogram": (C.c_int, [vp, C.c_int, vp, sz, sz, u32p, f64p, C.c_uint32, f64p, sz, vp, vp, vp, u8p]),
         "vmb_host_alloc": (vp, [sz]),
         "vmb_host_free": (None, [vp]),
         "vmb_ctx_last_stage_ms": (C.c_float, [vp, C.c_int]),

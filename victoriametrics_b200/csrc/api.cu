@@ -1882,6 +1882,7 @@ extern "C" int vmb_eval_rollup_aggr_device(vmb_ctx* ctx, const vmb_blocks* b, in
 #include "aggr_order.inc"
 #include "transform.inc"
 #include "range_transform.inc"
+#include "histogram.inc"
 
 // ------------------------------------------------------------------------------------------------ batched host encoder
 #include <atomic>

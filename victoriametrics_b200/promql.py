@@ -567,6 +567,43 @@ def transform_range(name, dev_ptr, nrows, points, *scalar_args, step=None, ctx=N
     return kept[:nrows].astype(bool) if kept is not None else None
 
 
+HISTOGRAM_FUNCS = {"histogram_quantile": 0, "histogram_quantiles": 0, "histogram_share": 1, "histogram_fraction": 2,
+                   "histogram_avg": 3, "histogram_stddev": 4, "histogram_stdvar": 5}
+_HISTOGRAM_NARGS = {"histogram_quantile": 1, "histogram_share": 1, "histogram_fraction": 2}
+
+
+def histogram(name, vals_dev_ptr, nrows, points, group_ids, les, ngroups, out_dev_ptr, *scalar_args, lower_dev_ptr=None,
+              upper_dev_ptr=None, ctx=None):
+    """The histogram functions over `le` buckets (transform.go:634-1169, vmb_histogram) on a DEVICE matrix [nrows x points] of
+    bucket series.  group_ids: the dense id of every row's label set without `le`, 0xffffffff for a row without a parsable `le`;
+    les: every row's parsed `le`.  scalar_args (numbers or per-point arrays, getScalar): histogram_quantile(phi),
+    histogram_quantiles(phi, ...), histogram_share(le), histogram_fraction(lower, upper); none for histogram_avg / stddev / stdvar.
+    -> out_dev_ptr [ngroups x points] (histogram_quantiles: [len(phis) x ngroups x points], phi-major); lower_dev_ptr /
+    upper_dev_ptr (histogram_quantile and histogram_share, both or neither): the boundsLabel series [ngroups x points].
+    Returns the np.bool_ mask of the output rows -- out rows, then lower, then upper -- that hold a value (removeEmptySeries)."""
+    ctx = ctx or _lib.default_context()
+    name = name.lower()
+    g = np.ascontiguousarray(group_ids, dtype=np.uint32)
+    le = np.ascontiguousarray(les, dtype=np.float64)
+    if g.size != int(nrows) or le.size != int(nrows):
+        raise ValueError("%s: need one group id and one le per row (%d rows)" % (name, nrows))
+    want = len(scalar_args) if name == "histogram_quantiles" else _HISTOGRAM_NARGS.get(name, 0)
+    if len(scalar_args) != want or (name == "histogram_quantiles" and not want):
+        raise ValueError("%s: unexpected number of scalar args: %d" % (name, len(scalar_args)))
+    args = None
+    if want:
+        args = np.ascontiguousarray(np.concatenate([np.broadcast_to(np.asarray(a, dtype=np.float64), (points,)) for a in scalar_args]))
+    bounds = lower_dev_ptr is not None or upper_dev_ptr is not None
+    nout = (want if name == "histogram_quantiles" else 1) * int(ngroups) + (2 * int(ngroups) if bounds else 0)
+    flags = np.zeros(max(nout, 1), dtype=np.uint8)
+    ptr = lambda p: C.c_void_p(int(p)) if p is not None else None
+    check(lib().vmb_histogram(ctx.h, HISTOGRAM_FUNCS[name], C.c_void_p(int(vals_dev_ptr)), int(nrows), int(points),
+                              g.ctypes.data_as(_lib.u32p), le.ctypes.data_as(_lib.f64p), int(ngroups),
+                              args.ctypes.data_as(_lib.f64p) if args is not None else None, 0 if args is None else args.size,
+                              C.c_void_p(int(out_dev_ptr)), ptr(lower_dev_ptr), ptr(upper_dev_ptr), flags.ctypes.data_as(_lib.u8p)))
+    return flags[:nout].astype(bool)
+
+
 MATRIX_AGGR_FUNCS = {n: i for i, n in enumerate(
     ["sum", "sum2", "min", "max", "avg", "count", "group", "geomean", "stddev", "stdvar", "share", "zscore"])}
 
