@@ -7,6 +7,7 @@
 #include <math.h>
 #include <string.h>
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -327,9 +328,13 @@ int vmo_check_timestamps_bounds(const int64_t* ts, size_t n, int64_t tmin, int64
 typedef size_t (*ref_compress_fn)(void*, size_t, const void*, size_t, int);
 typedef size_t (*ref_decompress_fn)(void*, size_t, const void*, size_t);
 typedef unsigned (*ref_iserr_fn)(size_t);
+typedef size_t (*ref_compress_params_fn)(void*, size_t, const void*, size_t, const int*, int);
+typedef size_t (*ref_compress_seq_fn)(void*, size_t, const void*, size_t, const unsigned*, size_t, const int*, int);
 static ref_compress_fn g_ref_compress;
 static ref_decompress_fn g_ref_decompress;
 static ref_compress_fn g_ref_compress_ck;
+static ref_compress_params_fn g_ref_compress_params;
+static ref_compress_seq_fn g_ref_compress_seq;
 static ref_iserr_fn g_ref_iserr;
 static int g_ref_state;  // 0 = not tried, 1 = ok, -1 = unavailable
 
@@ -349,12 +354,19 @@ static void load_ref() {
     g_ref_compress = (ref_compress_fn)dlsym(h, "ref_zstd_compress");
     g_ref_decompress = (ref_decompress_fn)dlsym(h, "ref_zstd_decompress");
     g_ref_compress_ck = (ref_compress_fn)dlsym(h, "ref_zstd_compress_checksum");
+    g_ref_compress_params = (ref_compress_params_fn)dlsym(h, "ref_zstd_compress_params");
+    g_ref_compress_seq = (ref_compress_seq_fn)dlsym(h, "ref_zstd_compress_sequences");
     g_ref_iserr = (ref_iserr_fn)dlsym(h, "ref_zstd_is_error");
     if (g_ref_compress && g_ref_decompress && g_ref_iserr) g_ref_state = 1;
 }
 int vmo_zstd_ref_available(void) {
     load_ref();
     return g_ref_state == 1;
+}
+// the frame factory (ref_zstd_compress_params / ref_zstd_compress_sequences): absent from an oracle/_ref built by an older
+// recipe, which still serves everything else
+int vmo_zstd_ref_factory_available(void) {
+    return vmo_zstd_ref_available() && g_ref_compress_params && g_ref_compress_seq;
 }
 int64_t vmo_zstd_ref_compress(uint8_t* dst, size_t cap, const uint8_t* src, size_t n, int level) {
     load_ref();
@@ -366,6 +378,21 @@ int64_t vmo_zstd_ref_compress(uint8_t* dst, size_t cap, const uint8_t* src, size
 int64_t vmo_zstd_ref_compress_checksum(uint8_t* dst, size_t cap, const uint8_t* src, size_t n, int level) {
     if (!vmo_zstd_ref_available() || !g_ref_compress_ck) return VMO_ERR_NO_ZSTD_REF;
     size_t r = g_ref_compress_ck(dst, cap, src, n, level);
+    if (g_ref_iserr(r)) return VMO_ERR_ZSTD;
+    return (int64_t)r;
+}
+// ZSTD_compress2 after ZSTD_CCtx_setParameter of each (param, value) pair in kv[0 .. 2 * nkv)
+int64_t vmo_zstd_ref_compress_params(uint8_t* dst, size_t cap, const uint8_t* src, size_t n, const int* kv, int nkv) {
+    if (!vmo_zstd_ref_factory_available()) return VMO_ERR_NO_ZSTD_REF;
+    size_t r = g_ref_compress_params(dst, cap, src, n, kv, nkv);
+    if (g_ref_iserr(r)) return VMO_ERR_ZSTD;
+    return (int64_t)r;
+}
+// ZSTD_compressSequences, explicit block delimiters: seq = nseq (offset, literal length, match length) triples
+int64_t vmo_zstd_ref_compress_sequences(uint8_t* dst, size_t cap, const uint8_t* src, size_t n, const uint32_t* seq, size_t nseq,
+                                        const int* kv, int nkv) {
+    if (!vmo_zstd_ref_factory_available()) return VMO_ERR_NO_ZSTD_REF;
+    size_t r = g_ref_compress_seq(dst, cap, src, n, seq, nseq, kv, nkv);
     if (g_ref_iserr(r)) return VMO_ERR_ZSTD;
     return (int64_t)r;
 }
@@ -423,8 +450,12 @@ int vmo_unmarshal_int64_array(int64_t* dst, const uint8_t* src, size_t src_len, 
     switch (mt) {
         case 4:
         case 1: {
-            int64_t cs = vmo_zstd_content_size(src, src_len);
+            // Frame_Content_Size, or for a frame without one (klauspost/compress omits it below 256 bytes) the bound of its
+            // content from the block headers, capped at 10 bytes per row (the varint decode rejects anything longer);
+            // the decoded length is what the frame produced
+            int64_t cs = vmo_zstd_content_bound(src, src_len);
             if (cs < 0) return VMO_ERR_ZSTD;
+            if (vmo_zstd_content_size(src, src_len) < 0) cs = std::min<int64_t>(cs, (int64_t)n * 10);
             std::vector<uint8_t> bb((size_t)cs + 8);
             int64_t r = vmo_zstd_decompress(bb.data(), (size_t)cs, src, src_len);
             if (r < 0) return VMO_ERR_ZSTD;

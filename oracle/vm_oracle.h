@@ -69,11 +69,20 @@ int vmo_unmarshal_int64_array(int64_t* dst, const uint8_t* src, size_t src_len, 
 /* own restatement of the zstd frame format (RFC 8878); returns regenerated size or <0 */
 int64_t vmo_zstd_decompress(uint8_t* dst, size_t cap, const uint8_t* src, size_t src_len);
 int64_t vmo_zstd_content_size(const uint8_t* src, size_t src_len);
+/* Frame_Content_Size, or for a frame without one an upper bound of its content from the block headers */
+int64_t vmo_zstd_content_bound(const uint8_t* src, size_t src_len);
 /* libzstd 1.5.7 (the reference's own) through oracle/_ref/libzstd_ref.so */
 int vmo_zstd_ref_available(void);
 int64_t vmo_zstd_ref_compress(uint8_t* dst, size_t cap, const uint8_t* src, size_t n, int level);
 int64_t vmo_zstd_ref_decompress(uint8_t* dst, size_t cap, const uint8_t* src, size_t n);
 int64_t vmo_zstd_ref_compress_checksum(uint8_t* dst, size_t cap, const uint8_t* src, size_t n, int level); /* with Content_Checksum */
+/* both functions below are present (an oracle/_ref built by an older recipe lacks them) */
+int vmo_zstd_ref_factory_available(void);
+/* ZSTD_compress2 after ZSTD_CCtx_setParameter(kv[2i], kv[2i+1]) for i < nkv */
+int64_t vmo_zstd_ref_compress_params(uint8_t* dst, size_t cap, const uint8_t* src, size_t n, const int* kv, int nkv);
+/* ZSTD_compressSequences with explicit block delimiters: nseq (offset, literal length, match length) triples */
+int64_t vmo_zstd_ref_compress_sequences(uint8_t* dst, size_t cap, const uint8_t* src, size_t n, const uint32_t* seq, size_t nseq,
+                                        const int* kv, int nkv);
 
 /* ---- lib/decimal/decimal.go ---- */
 double vmo_pow10(int n); /* Go math.Pow10 */

@@ -9,6 +9,7 @@
 // ZSTD_compressCCtx at levels -5..5 on the codec's varint streams must decode byte-identically).
 #include <string.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "vm_oracle.h"
@@ -494,6 +495,7 @@ struct FrameHdr {
     bool has_fcs;
     uint64_t fcs;
     bool checksum;
+    uint64_t block_max;  // Block_Maximum_Size = min(Window_Size, 128 KiB)
 };
 
 FrameHdr parse_frame_header(const uint8_t* src, size_t len) {
@@ -524,7 +526,13 @@ FrameHdr parse_frame_header(const uint8_t* src, size_t len) {
     for (int i = 0; i < fcs_size; i++) fcs |= (uint64_t)src[pos + i] << (8 * i);
     if (fcs_size == 2) fcs += 256;
     pos += fcs_size;
-    return FrameHdr{pos, fcs_size != 0, fcs, checksum};
+    uint64_t window = fcs;  // Single_Segment_Flag: the window is the content
+    if (!single) {
+        // Window_Descriptor (RFC 8878 3.1.1.1.2)
+        const int wlog = 10 + (src[5] >> 3);
+        window = (1ull << wlog) + ((1ull << wlog) / 8) * (src[5] & 7);
+    }
+    return FrameHdr{pos, fcs_size != 0, fcs, checksum, std::min<uint64_t>(window, 128 << 10)};
 }
 
 }  // namespace
@@ -536,6 +544,33 @@ int64_t vmo_zstd_content_size(const uint8_t* src, size_t len) {
         FrameHdr h = parse_frame_header(src, len);
         if (!h.has_fcs) return VMO_ERR_ZSTD;
         return (int64_t)h.fcs;
+    } catch (Err&) {
+        return VMO_ERR_ZSTD;
+    }
+}
+
+// Frame_Content_Size when the frame has one; otherwise an upper bound of the content from the block headers (Raw and RLE
+// blocks exactly, a Compressed block at most Block_Maximum_Size).  Errors when the block headers run past the frame.
+int64_t vmo_zstd_content_bound(const uint8_t* src, size_t len) {
+    try {
+        FrameHdr h = parse_frame_header(src, len);
+        if (h.has_fcs) return (int64_t)h.fcs;
+        uint64_t bound = 0;
+        size_t pos = h.hdr_size;
+        for (;;) {
+            if (pos + 3 > len) throw Err();
+            uint32_t bh = src[pos] | ((uint32_t)src[pos + 1] << 8) | ((uint32_t)src[pos + 2] << 16);
+            pos += 3;
+            int type = (bh >> 1) & 3;
+            size_t bsize = bh >> 3;
+            if (type == 3) throw Err();
+            size_t stored = type == 1 ? 1 : bsize;
+            if (pos + stored > len) throw Err();
+            pos += stored;
+            bound += type == 2 ? h.block_max : bsize;
+            if (bh & 1) break;
+        }
+        return (int64_t)bound;
     } catch (Err&) {
         return VMO_ERR_ZSTD;
     }
@@ -566,7 +601,9 @@ int64_t vmo_zstd_decompress(uint8_t* dst, size_t cap, const uint8_t* src, size_t
                 o += bsize;
             } else if (type == 2) {
                 if (pos + bsize > len) throw Err();
-                o += decode_block(fc, dst, o, cap, src + pos, bsize);
+                size_t regen = decode_block(fc, dst, o, cap, src + pos, bsize);
+                if (!h.has_fcs && regen > h.block_max) throw Err();  // libzstd: a block larger than the window is corrupt
+                o += regen;
                 pos += bsize;
             } else {
                 throw Err();

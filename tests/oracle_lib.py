@@ -68,9 +68,14 @@ def lib():
         "vmo_zstd_decompress": (C.c_int64, [u8p, sz, u8p, sz]),
         "vmo_zstd_content_size": (C.c_int64, [u8p, sz]),
         "vmo_zstd_ref_available": (C.c_int, []),
+        "vmo_zstd_ref_factory_available": (C.c_int, []),
         "vmo_zstd_ref_compress": (C.c_int64, [u8p, sz, u8p, sz, C.c_int]),
         "vmo_zstd_ref_decompress": (C.c_int64, [u8p, sz, u8p, sz]),
         "vmo_zstd_ref_compress_checksum": (C.c_int64, [u8p, sz, u8p, sz, C.c_int]),
+        "vmo_zstd_ref_compress_params": (C.c_int64, [u8p, sz, u8p, sz, C.POINTER(C.c_int), C.c_int]),
+        "vmo_zstd_ref_compress_sequences": (C.c_int64, [u8p, sz, u8p, sz, C.POINTER(C.c_uint32), sz,
+                                                        C.POINTER(C.c_int), C.c_int]),
+        "vmo_zstd_content_bound": (C.c_int64, [u8p, sz]),
         "vmo_pow10": (C.c_double, [C.c_int]),
         "vmo_decimal_to_float": (None, [f64p, i64p, sz, C.c_int16]),
         "vmo_float_to_decimal": (C.c_int16, [i64p, f64p, sz]),
@@ -190,8 +195,9 @@ def unmarshal_int64_array(src, mt, first, n):
 
 
 def zstd_decompress(src):
+    """the oracle's own decoder, into Frame_Content_Size or (without one) the bound of the content from the block headers"""
     src = np.ascontiguousarray(src, dtype=np.uint8)
-    cs = lib().vmo_zstd_content_size(_u8(src), len(src))
+    cs = lib().vmo_zstd_content_bound(_u8(src), len(src))
     if cs < 0:
         return cs, None
     dst = np.empty(cs + 8, dtype=np.uint8)
@@ -218,6 +224,54 @@ def zstd_ref_compress_checksum(src, level):
     if n < 0:
         raise RuntimeError("zstd ref compress (checksum) rc=%d" % n)
     return dst[:n].copy()
+
+
+# ZSTD_cParameter values of libzstd 1.5.7 (zstd.h; the experimental ones under ZSTD_STATIC_LINKING_ONLY)
+ZSTD_C = {"compressionLevel": 100, "windowLog": 101, "hashLog": 102, "chainLog": 103, "searchLog": 104, "minMatch": 105,
+          "targetLength": 106, "strategy": 107, "targetCBlockSize": 130, "contentSizeFlag": 200, "checksumFlag": 201,
+          "literalCompressionMode": 1002, "maxBlockSize": 1015}
+ZSTD_LCM_HUFFMAN, ZSTD_LCM_UNCOMPRESSED = 1, 2  # ZSTD_ParamSwitch_e values of literalCompressionMode
+
+
+def _kv(params):
+    kv = []
+    for k, v in (params or {}).items():
+        kv += [ZSTD_C[k], int(v)]
+    return (C.c_int * max(len(kv), 1))(*kv), len(kv) // 2
+
+
+def zstd_ref_compress_params(src, **params):
+    """ZSTD_compress2 with ZSTD_CCtx_setParameter(name, value) for each keyword (names as in ZSTD_C)"""
+    src = np.ascontiguousarray(src, dtype=np.uint8)
+    dst = np.empty(len(src) + (len(src) >> 7) + 1024, dtype=np.uint8)
+    kv, nkv = _kv(params)
+    n = lib().vmo_zstd_ref_compress_params(_u8(dst), dst.size, _u8(src), len(src), kv, nkv)
+    if n < 0:
+        raise RuntimeError("zstd ref compress %s rc=%d" % (params, n))
+    return dst[:n].copy()
+
+
+def zstd_ref_compress_sequences(src, seqs, **params):
+    """ZSTD_compressSequences with explicit block delimiters.  seqs: (offset, literal length, match length) triples over
+    src; (0, ll, 0) closes a block with ll trailing literals.  Repeat offsets are resolved by the compressor."""
+    src = np.ascontiguousarray(src, dtype=np.uint8)
+    s = np.ascontiguousarray(np.asarray(seqs, dtype=np.uint32).reshape(-1, 3))
+    dst = np.empty(len(src) + (len(src) >> 7) + 1024, dtype=np.uint8)
+    params.setdefault("minMatch", 3)  # (the validation rejects matches shorter than minMatch)
+    kv, nkv = _kv(params)
+    n = lib().vmo_zstd_ref_compress_sequences(_u8(dst), dst.size, _u8(src), len(src), s.ctypes.data_as(C.POINTER(C.c_uint32)),
+                                              len(s), kv, nkv)
+    if n < 0:
+        raise RuntimeError("zstd ref compress_sequences rc=%d" % n)
+    return dst[:n].copy()
+
+
+def zstd_ref_decompress_rc(src, cap):
+    """libzstd's ZSTD_decompressDCtx into cap bytes: (length or a negative rc, bytes or None)"""
+    src = np.ascontiguousarray(src, dtype=np.uint8)
+    dst = np.empty(cap + 8, dtype=np.uint8)
+    n = lib().vmo_zstd_ref_decompress(_u8(dst), cap, _u8(src), len(src))
+    return (n, dst[:n].copy()) if n >= 0 else (n, None)
 
 
 def zstd_ref_decompress(src, cap):

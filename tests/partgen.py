@@ -2,12 +2,15 @@
 flushIndexData): timestamps.bin / values.bin hold the marshaled columns (identical consecutive timestamp payloads stored
 once), index.bin the zstd-compressed runs of 81-byte block headers (a run is flushed before it would exceed maxBlockSize),
 metaindex.bin one zstd frame of 56-byte rows.  Compression = the reference's libzstd (oracle/_ref), payloads = the oracle's
-MarshalData -- nothing of the product is on this side except the struct layouts the checks compare against."""
+MarshalData -- nothing of the product is on this side except the struct layouts the checks compare against.
+pure_go=True writes the frames in the header layout of the reference's builds without cgo (klauspost/compress): below
+256 bytes they carry no Frame_Content_Size, up to 1024 bytes a Window_Descriptor beside it."""
 import struct
 
 import numpy as np
 
 import oracle_lib as O
+import zstd_shapes
 
 MAX_BLOCK_SIZE = 64 * 1024  # block.go:18
 
@@ -32,9 +35,22 @@ def pack_metaindex_row(tsid, count, min_ts, max_ts, off, size):
     return tsid + struct.pack(">IQQQI", count, zz(min_ts), zz(max_ts), off, size)  # metaindex_row.go:61
 
 
-def write_part(series, level=1, max_index_block=MAX_BLOCK_SIZE):
+def pure_go_columns(block, level):
+    """rewrite the zstd columns (MarshalType 1 / 4) of an OBlock in place as the pure-Go writer frames them"""
+    for d, mt in (("tdata", "tmt"), ("vdata", "vmt")):
+        if getattr(block, mt) in (1, 4):
+            raw = O.zstd_ref_decompress(getattr(block, d), block.rows * 10 + 16)
+            setattr(block, d, zstd_shapes.pure_go_frame(raw, compressionLevel=level))
+
+
+def write_part(series, level=1, max_index_block=MAX_BLOCK_SIZE, pure_go=False):
     """series: list of (tsid bytes, [OBlock, ...]) sorted by tsid, blocks by min timestamp.
-    -> dict(metaindex_bin, index_bin, timestamps_bin, values_bin, headers=[(tsid, header dict)], index_blocks=n)"""
+    -> dict(metaindex_bin, index_bin, timestamps_bin, values_bin, headers=[(tsid, header dict)], index_blocks=n)
+    pure_go: every frame in the pure-Go writer's header layout (the blocks' zstd columns are rewritten in place)"""
+    def compress(raw):
+        raw = np.frombuffer(bytes(raw), dtype=np.uint8)
+        return (zstd_shapes.pure_go_frame(raw, compressionLevel=level) if pure_go else O.zstd_ref_compress(raw, level)).tobytes()
+
     tsb, vsb, index_bin, metaindex = bytearray(), bytearray(), bytearray(), bytearray()
     headers = []
     cur = bytearray()
@@ -46,7 +62,7 @@ def write_part(series, level=1, max_index_block=MAX_BLOCK_SIZE):
         nonlocal cur, mr, n_index_blocks
         if not cur:
             return
-        comp = O.zstd_ref_compress(np.frombuffer(bytes(cur), dtype=np.uint8), level).tobytes()
+        comp = compress(cur)
         metaindex.extend(pack_metaindex_row(mr["tsid"], mr["count"], mr["min_ts"], mr["max_ts"], len(index_bin), len(comp)))
         index_bin.extend(comp)
         cur = bytearray()
@@ -55,6 +71,8 @@ def write_part(series, level=1, max_index_block=MAX_BLOCK_SIZE):
 
     for tsid, blocks in series:
         for b in blocks:
+            if pure_go:
+                pure_go_columns(b, level)
             h = b.header()
             td = b.tdata.tobytes()
             if prev_ts is not None and len(prev_ts) > 0 and td == prev_ts:
@@ -76,6 +94,6 @@ def write_part(series, level=1, max_index_block=MAX_BLOCK_SIZE):
             mr["max_ts"] = max(mr["max_ts"], h["max_ts"])
             headers.append((tsid, h))
     flush()
-    mi = O.zstd_ref_compress(np.frombuffer(bytes(metaindex), dtype=np.uint8), level).tobytes()
+    mi = compress(metaindex)
     return dict(metaindex_bin=mi, index_bin=bytes(index_bin), timestamps_bin=bytes(tsb), values_bin=bytes(vsb), headers=headers,
                 index_blocks=n_index_blocks, metaindex_raw=bytes(metaindex))

@@ -773,11 +773,11 @@ static int run_zstd(vmb_ctx* ctx, const vmb_blocks* b, int32_t** d_zstatus_out, 
 }
 
 // runs zstd + column decode + series assembly into `s` (whose buffers are already allocated)
-// zstd_done: the zstd stage of the upload this (sub-)batch belongs to ran already, its status array is d_zstatus_in and block k of
-// `b` is block d_blk_map[k] of that upload
+// zstd_done: the zstd stage of the upload this (sub-)batch belongs to ran already, its status array is d_zstatus_in, its column
+// infos (with the lengths the frames produced) d_zcols_in, and block k of `b` is block d_blk_map[k] of that upload
 static int run_decode(vmb_ctx* ctx, const vmb_blocks* b, vmb_series* s, int64_t tr_min, int64_t tr_max, uint32_t flags,
                       unsigned int* d_failed, bool zstd_done = false, int32_t* d_zstatus_in = nullptr,
-                      const uint32_t* d_blk_map = nullptr) {
+                      const uint32_t* d_blk_map = nullptr, const ColInfo* d_zcols_in = nullptr) {
     cudaStream_t st = ctx->stream;
     if (ctx->timing && !zstd_done) CU(cudaEventRecord(ctx->ev[ST_ZSTD], st));
     int32_t* d_zstatus = d_zstatus_in;
@@ -793,6 +793,7 @@ static int run_decode(vmb_ctx* ctx, const vmb_blocks* b, vmb_series* s, int64_t 
     D.payload = b->d_payload;
     D.scratch = (const uint8_t*)ctx->zscratch.p;
     D.zstd_status = d_zstatus;
+    D.zstd_cols = zstd_done ? d_zcols_in : b->d_cols;
     D.blk_map = d_blk_map;
     D.row_off = b->d_row_off;
     D.ts_out = s->d_ts;
@@ -1649,7 +1650,7 @@ static int run_unfused_subset(vmb_ctx* ctx, const vmb_blocks* b, const std::vect
     bv.d_payload = b->d_payload;
     vmb_series view;
     if ((rc = column_cache_view(ctx, &bv, &view))) return rc;
-    rc = run_decode(ctx, &bv, &view, tr_min, tr_max, 0, c.d_failed, true, d_zstatus, L.extra_at(da, 0));
+    rc = run_decode(ctx, &bv, &view, tr_min, tr_max, 0, c.d_failed, true, d_zstatus, L.extra_at(da, 0), b->d_cols);
     if (!rc) rc = run_rollup(ctx, &view, cfg, points, d_out, c.d_scanned, dense_rows ? nullptr : L.extra_at(da, 1), false);
     cudaError_t e = cudaStreamSynchronize(st);  // `hs` goes out of scope
     if (!rc && e != cudaSuccess) {

@@ -27,7 +27,8 @@ enum : uint8_t {
 
 struct ColInfo {            // one per column (2 per block: [2*b] timestamps, [2*b+1] values)
     uint64_t scratch_off;   // where the decompressed varint bytes go inside the zstd scratch arena
-    uint32_t content_size;  // decompressed size (frame header)
+    uint32_t content_size;  // decompressed size: Frame_Content_Size; without one, the host's bound until the serial
+                            // decoder stores the length the frame produced (in the device copy)
     uint8_t kind;           // VMB_ZK_*
     uint8_t _pad[3];
     uint32_t nseq;          // VMB_ZK_HUF: Number_of_Sequences of the block (read by the host plan from the section header)

@@ -212,6 +212,7 @@ struct DecodeParams {
     const uint8_t* payload;
     const uint8_t* scratch;       // zstd output arena
     const int32_t* zstd_status;   // per column (2*nblocks) or nullptr
+    const ColInfo* zstd_cols;     // the column infos the zstd stage ran on: their content_size is the length each frame produced
     const uint32_t* blk_map;      // sub-batch of a larger upload: block b is block blk_map[b] of the batch zstd_status belongs to
     const uint64_t* row_off;      // per block: first row in the dense columns
     int64_t* ts_out;
@@ -234,9 +235,9 @@ __global__ void __launch_bounds__(128) k_decode_columns(DecodeParams P) {
         const uint64_t ro = P.row_off[b];
         int rc = 0;
         uint32_t lo = 0, hi = 0;
+        const uint32_t zb = P.blk_map ? P.blk_map[b] : b;
         if (d.rows == 0 || d.rows > 16384u) rc = VMB_ERR_ROWS;  // block.go:262, block_header.go:233
         if (!rc && P.zstd_status) {
-            const uint32_t zb = P.blk_map ? P.blk_map[b] : b;
             int z0 = P.zstd_status[2 * zb], z1 = P.zstd_status[2 * zb + 1];
             if (z0) rc = z0;
             else if (z1) rc = z1;
@@ -245,7 +246,7 @@ __global__ void __launch_bounds__(128) k_decode_columns(DecodeParams P) {
             // ---- timestamps (encoding.UnmarshalTimestamps encoding.go:90)
             const ColInfo ci = P.cols[2 * b];
             const uint8_t* src = ci.kind == VMB_ZK_NONE ? P.payload + d.ts_off : P.scratch + ci.scratch_off;
-            uint32_t len = ci.kind == VMB_ZK_NONE ? d.ts_size : ci.content_size;
+            uint32_t len = ci.kind == VMB_ZK_NONE ? d.ts_size : P.zstd_cols[2 * zb].content_size;
             TsEmit te;
             const bool needs_validation = d.precision_bits >= 64 && (d.ts_mt == 5 || d.ts_mt == 6);  // encoding.go:46
             te.init(P.ts_out + ro, P.tr_min, P.tr_max, needs_validation);
@@ -296,7 +297,7 @@ __global__ void __launch_bounds__(128) k_decode_columns(DecodeParams P) {
             // ---- values (encoding.UnmarshalValues encoding.go:111 + decimal.AppendDecimalToFloat)
             const ColInfo ci = P.cols[2 * b + 1];
             const uint8_t* src = ci.kind == VMB_ZK_NONE ? P.payload + d.val_off : P.scratch + ci.scratch_off;
-            uint32_t len = ci.kind == VMB_ZK_NONE ? d.val_size : ci.content_size;
+            uint32_t len = ci.kind == VMB_ZK_NONE ? d.val_size : P.zstd_cols[2 * zb + 1].content_size;
             ValEmit ve;
             const bool as_int = (P.flags & VMB_DECODE_VALUES_AS_INT64) != 0;
             ve.init(as_int ? (void*)((int64_t*)P.val_out + ro) : (void*)((double*)P.val_out + ro), d.scale, as_int);

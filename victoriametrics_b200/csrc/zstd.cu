@@ -526,6 +526,7 @@ struct FrameHdr {
     uint32_t hdr_size;
     bool has_fcs, checksum;
     unsigned long long fcs;
+    unsigned long long block_max;  // Block_Maximum_Size = min(Window_Size, 128 KiB) (RFC 8878 3.1.1.1.2)
 };
 
 __host__ __device__ inline bool parse_frame_header(FrameHdr* h, const uint8_t* src, uint32_t len) {
@@ -556,6 +557,12 @@ __host__ __device__ inline bool parse_frame_header(FrameHdr* h, const uint8_t* s
     h->hdr_size = pos;
     h->has_fcs = fcs_size != 0;
     h->fcs = fcs;
+    unsigned long long window = fcs;  // Single_Segment: Window_Size = Frame_Content_Size
+    if (!single) {
+        const uint32_t wd = src[5], wlog = 10 + (wd >> 3);
+        window = (1ull << wlog) + ((1ull << wlog) >> 3) * (wd & 7);
+    }
+    h->block_max = window < (128u << 10) ? window : (128u << 10);
     return true;
 }
 
@@ -617,10 +624,12 @@ __device__ unsigned long long xxh64(const uint8_t* p, unsigned long long len) {
     return h;
 }
 
-__device__ bool decode_frame_serial(SerialWs* ws, uint8_t* out, uint32_t out_cap, uint8_t* litbuf, const uint8_t* src,
-                                    uint32_t len) {
+// A frame with a Frame_Content_Size must fill out_cap exactly; one without it may produce up to out_cap bytes, and each of its
+// Compressed blocks at most Block_Maximum_Size (what libzstd enforces).  Returns the bytes produced, or -1.
+__device__ long long decode_frame_serial(SerialWs* ws, uint8_t* out, uint32_t out_cap, uint8_t* litbuf, const uint8_t* src,
+                                         uint32_t len) {
     FrameHdr h;
-    if (!parse_frame_header(&h, src, len)) return false;
+    if (!parse_frame_header(&h, src, len)) return -1;
     uint32_t pos = h.hdr_size;
     long long o = 0;
     ws->have_ll = ws->have_ml = ws->have_of = ws->have_huf = 0;
@@ -628,40 +637,42 @@ __device__ bool decode_frame_serial(SerialWs* ws, uint8_t* out, uint32_t out_cap
     ws->rep[1] = 4;
     ws->rep[2] = 8;
     for (;;) {
-        if (pos + 3 > len) return false;
+        if (pos + 3 > len) return -1;
         uint32_t bh = src[pos] | ((uint32_t)src[pos + 1] << 8) | ((uint32_t)src[pos + 2] << 16);
         pos += 3;
         bool last = bh & 1;
         int type = (bh >> 1) & 3;
         uint32_t bsize = bh >> 3;
         if (type == 0) {
-            if (pos + bsize > len || o + bsize > out_cap) return false;
+            if (pos + bsize > len || o + bsize > out_cap) return -1;
             for (uint32_t k = 0; k < bsize; k++) out[o + k] = src[pos + k];
             pos += bsize;
             o += bsize;
         } else if (type == 1) {
-            if (pos + 1 > len || o + bsize > out_cap) return false;
+            if (pos + 1 > len || o + bsize > out_cap) return -1;
             for (uint32_t k = 0; k < bsize; k++) out[o + k] = src[pos];
             pos += 1;
             o += bsize;
         } else if (type == 2) {
-            if (pos + bsize > len) return false;
+            if (pos + bsize > len) return -1;
+            const long long o0 = o;
             o = decode_block_serial(ws, out, o, out_cap, litbuf, src + pos, bsize);
-            if (o < 0) return false;
+            if (o < 0) return -1;
+            if (!h.has_fcs && (unsigned long long)(o - o0) > h.block_max) return -1;
             pos += bsize;
         } else {
-            return false;
+            return -1;
         }
         if (last) break;
     }
-    if ((unsigned long long)o != (unsigned long long)out_cap) return false;
+    if (h.has_fcs && (unsigned long long)o != (unsigned long long)out_cap) return -1;
     if (h.checksum) {
-        if (pos + 4 > len) return false;
+        if (pos + 4 > len) return -1;
         const uint32_t want = src[pos] | ((uint32_t)src[pos + 1] << 8) | ((uint32_t)src[pos + 2] << 16) | ((uint32_t)src[pos + 3] << 24);
-        if ((uint32_t)xxh64(out, (unsigned long long)o) != want) return false;  // corrupted content
+        if ((uint32_t)xxh64(out, (unsigned long long)o) != want) return -1;  // corrupted content
         pos += 4;
     }
-    return pos == len;
+    return pos == len ? o : -1;
 }
 
 }  // namespace
@@ -669,7 +680,7 @@ __device__ bool decode_frame_serial(SerialWs* ws, uint8_t* out, uint32_t out_cap
 // ------------------------------------------------------------------------------------------------ kernels
 struct ZstdParams {
     const vmb_block_desc* descs;
-    const ColInfo* cols;
+    ColInfo* cols;         // (k_zstd_serial writes content_size of frames without Frame_Content_Size)
     const uint8_t* payload;
     uint8_t* scratch;      // decompressed varint bytes
     uint8_t* lit;          // literal arena (same offsets as scratch) or nullptr
@@ -1550,9 +1561,13 @@ __global__ void k_zstd_serial(ZstdParams P, int mode) {
             const uint8_t* src;
             uint32_t len;
             col_src(P, col, &src, &len);
-            bool ok = P.lit && decode_frame_serial(ws, P.scratch + ci.scratch_off, ci.content_size,
-                                                   P.lit + ci.scratch_off, src, len);
-            P.status[col] = ok ? 0 : VMB_ERR_ZSTD;
+            const long long o = P.lit ? decode_frame_serial(ws, P.scratch + ci.scratch_off, ci.content_size,
+                                                            P.lit + ci.scratch_off, src, len)
+                                      : -1;
+            P.status[col] = o >= 0 ? 0 : VMB_ERR_ZSTD;
+            // a frame without Frame_Content_Size was given the host's bound of its content: what the column decoders read is
+            // the length it actually produced
+            if (o >= 0 && o != (long long)ci.content_size) P.cols[col].content_size = (uint32_t)o;
         }
     }
 }
@@ -1609,8 +1624,33 @@ void launch_zstd_serial(const ZstdParams& P, int mode, cudaStream_t st) {
 }
 
 // ---- host-side classification at upload time: reads only the frame / block / literals headers
+
+// A frame without Frame_Content_Size (klauspost/compress, the reference's writer in builds without cgo, omits it below 256
+// bytes): an upper bound of its content from the block headers.  Raw and RLE blocks are exact; a Compressed block
+// regenerates at most Block_Maximum_Size.  false: the block headers run past the end of the frame.
+static bool zstd_content_bound_host(const FrameHdr& h, const uint8_t* src, uint32_t len, unsigned long long* bound) {
+    unsigned long long b = 0;
+    uint32_t pos = h.hdr_size;
+    for (;;) {
+        if (pos + 3 > len) return false;
+        const uint32_t bh = src[pos] | ((uint32_t)src[pos + 1] << 8) | ((uint32_t)src[pos + 2] << 16);
+        pos += 3;
+        const uint32_t bsize = bh >> 3, type = (bh >> 1) & 3;
+        if (type == 3) return false;
+        const uint32_t stored = type == 1 ? 1u : bsize;
+        if ((unsigned long long)pos + stored > len) return false;
+        pos += stored;
+        b += type == 2 ? h.block_max : bsize;
+        if (bh & 1) break;
+    }
+    *bound = b;
+    return true;
+}
+
 // returns kind; fills content_size; *needs_lit = the literal arena is required for this column
 // content_bound = 0: a block payload, at most 10 bytes per row; else the caller's cap on Frame_Content_Size
+// A frame without Frame_Content_Size always takes the serial decoder, with content_size = the bound of its content; the
+// decoder replaces that with the length it produced.
 uint8_t zstd_classify_host(const uint8_t* src, uint32_t len, uint32_t rows, uint32_t* content_size, bool* needs_lit,
                            uint32_t* nseq, unsigned long long content_bound = 0) {
     *needs_lit = false;
@@ -1620,7 +1660,14 @@ uint8_t zstd_classify_host(const uint8_t* src, uint32_t len, uint32_t rows, uint
     if (!parse_frame_header(&h, src, len)) return VMB_ZK_BAD;
     // a valid payload holds rows-1 varints of <= 10 bytes
     unsigned long long bound = content_bound ? content_bound : (unsigned long long)rows * 10ull;
-    if (!h.has_fcs || h.fcs > bound) return VMB_ZK_BAD;
+    if (!h.has_fcs) {
+        unsigned long long cb;
+        if (!zstd_content_bound_host(h, src, len, &cb)) return VMB_ZK_BAD;
+        *content_size = (uint32_t)(cb < bound ? cb : bound);
+        *needs_lit = true;
+        return VMB_ZK_GENERIC;
+    }
+    if (h.fcs > bound) return VMB_ZK_BAD;
     *content_size = (uint32_t)h.fcs;
     uint32_t pos = h.hdr_size;
     if (pos + 3 > len) return VMB_ZK_BAD;
