@@ -442,7 +442,8 @@ int vmb_aggr_order(vmb_ctx* ctx, int func, const double* d_vals, size_t nseries,
                    uint32_t ngroups, const double* args, size_t nargs, double* d_out, unsigned char* row_nonempty,
                    unsigned char* row_selected);
 /* The histogram functions over Prometheus `le` buckets (app/vmselect/promql/transform.go:634-1169) on a DEVICE matrix d_buckets
- * [nrows x P], one bucket series per row; read only, it must not overlap an output.  `vmrange` buckets stay with the host.
+ * [nrows x P], one bucket series per row; read only, it must not overlap an output.  `vmrange` buckets go through
+ * vmb_vmrange_to_le (below) first, as every histogram_* of the reference does (vmrangeBucketsToLE).
  *   group_ids: HOST, one per row, the dense id of the row's label set without `le` (groupLeTimeseries :1097); UINT32_MAX for a row
  *              without an `le` label or whose `le` does not parse (:1102, :1106): it belongs to no group.
  *   les:       HOST, one per row, the parsed `le`.
@@ -470,6 +471,47 @@ enum vmb_hist_func { VMB_HF_QUANTILE = 0, VMB_HF_SHARE, VMB_HF_FRACTION, VMB_HF_
 int vmb_histogram(vmb_ctx* ctx, int func, const double* d_buckets, size_t nrows, size_t points, const uint32_t* group_ids,
                   const double* les, uint32_t ngroups, const double* args, size_t nargs, double* d_out, double* d_lower,
                   double* d_upper, unsigned char* out_nonempty);
+/* prometheus_buckets: vmrangeBucketsToLE (app/vmselect/promql/transform.go:494-632) on a DEVICE matrix d_buckets [nrows x P] of
+ * VictoriaMetrics histogram buckets (`vmrange="<start>...<end>"`); read only, it must not overlap d_out.  Labels stay with the
+ * host, which passes numbers and string ids:
+ *   group_ids: HOST, one per row: the dense id (< ngroups) of the row's label set without `vmrange` and `le`; VMB_VR_KEEP for a row
+ *              without `vmrange` but with a non-empty `le` (kept as it is, :510); UINT32_MAX for a row that is dropped: no
+ *              `vmrange` and no `le`, no "..." in it, or a start or end that strconv.ParseFloat rejects (:517-530).
+ *   starts, ends: HOST, one per row, the parsed start and end (read for grouped rows only).
+ *   start_keys, end_keys: HOST, one per row, ids of the start and end STRINGS: equal strings, equal ids; different strings,
+ *              different ids (the reference keys its maps by the strings, so `1e2` and `100` stay apart).
+ *   d_out:     [*nout x P]: the kept rows in input order, then the groups in ascending id, each in the reference's output order.
+ *   nout:      in: the capacity of d_out in rows; out: the rows needed.  d_out == NULL or too small: VMB_ERR_CAP, nothing else
+ *              written (a first call with d_out == NULL sizes d_out exactly).
+ *   out_src, out_kind, out_le: HOST, one per output row: the input row it comes from; enum vmb_vr_kind; the string id of its `le`
+ *              (start key for a gap row, end key for a bucket row; UINT32_MAX for a kept row, whose own `le` stays, and for a
+ *              +Inf row, whose `le` is "+Inf").
+ * Per group, sorted by end (the order of hg_sort_rows: Go's sort.Slice for up to 12 rows; for more than 12 rows with equal or NaN
+ * ends Go's pdqsort may order them otherwise), the rows are walked with the previous end starting at 0: a row without a value > 0
+ * is skipped; a start != the previous end adds a zero gap row with le = start unless that string was seen (it then names the
+ * source row, not the gap row); the row takes le = end, and an end string already seen merges the row into the row it names
+ * (mergeNonOverlappingTimeseries binary_op.go:367: at most 2 overlapping points, P > 2) instead of being output; a +Inf row
+ * follows unless the last end is +Inf.  Then every point runs count += v over the output rows, v > 0 and not NaN.  Bit-identical
+ * to the reference.  VMB_ERR_INVALID_ARG for a missing pointer, a group id >= ngroups other than VMB_VR_KEEP / UINT32_MAX, or
+ * nrows / points > 2^31 - 1, with the outputs untouched.  nrows == 0: *nout = 0. */
+#define VMB_VR_KEEP 0xfffffffeu
+enum vmb_vr_kind { VMB_VR_KEPT = 0, VMB_VR_BUCKET, VMB_VR_GAP, VMB_VR_INF };
+int vmb_vmrange_to_le(vmb_ctx* ctx, const double* d_buckets, size_t nrows, size_t points, const uint32_t* group_ids,
+                      const double* starts, const double* ends, const uint32_t* start_keys, const uint32_t* end_keys,
+                      uint32_t ngroups, double* d_out, size_t* nout, uint32_t* out_src, unsigned char* out_kind,
+                      uint32_t* out_le);
+/* buckets_limit(limit, buckets) (transform.go:386-483) on a DEVICE `le` matrix d_buckets [nrows x P], usually the d_out of
+ * vmb_vmrange_to_le in its order.  group_ids / les as in vmb_histogram: the dense id of the row's label set without `le`, UINT32_MAX
+ * for a row without a parsable `le` (dropped, :418-427).  limit <= 0: no rows; limit < 3 counts as 3.  A group of at most limit
+ * rows is kept in input order; a larger one is sorted by le (hg_sort_rows, as in vmb_histogram), every row gets hits = the sum
+ * over the points, in order, of v - v(previous row) (0 before the first), and the adjacent pair with the fewest hits is merged
+ * (the lower row dropped, its hits added to the next) until limit rows are left; the first and the last row stay.
+ *   out_rows:  HOST, the kept rows, groups in ascending id.  nout: in: the capacity of out_rows; out: the rows kept
+ *              (VMB_ERR_CAP when the capacity is too small; nrows always suffices).
+ * No matrix is written: vmb_histogram over d_buckets with UINT32_MAX for the rows not kept is histogram_*(buckets_limit(...)).
+ * Errors as vmb_vmrange_to_le. */
+int vmb_buckets_limit(vmb_ctx* ctx, const double* d_buckets, size_t nrows, size_t points, const uint32_t* group_ids,
+                      const double* les, uint32_t ngroups, int64_t limit, uint32_t* out_rows, size_t* nout);
 
 /* ---- multi-GPU: one process per GPU, the ONE exchange step of the path inside the library (SURVEY 8e) ------------------
  * aggr(rollup(m[d])) by (...): every rank folds its shard of the series into {values, counts}[G x P] (the per-worker

@@ -138,6 +138,9 @@ def lib():
         "vmb_transform": (C.c_int, [vp, C.c_int, vp, sz, sz, f64p, f64p]),
         "vmb_transform_range": (C.c_int, [vp, C.c_int, vp, sz, sz, f64p, sz, u8p]),
         "vmb_histogram": (C.c_int, [vp, C.c_int, vp, sz, sz, u32p, f64p, C.c_uint32, f64p, sz, vp, vp, vp, u8p]),
+        "vmb_vmrange_to_le": (C.c_int, [vp, vp, sz, sz, u32p, f64p, f64p, u32p, u32p, C.c_uint32, vp, C.POINTER(sz), u32p, u8p,
+                                        u32p]),
+        "vmb_buckets_limit": (C.c_int, [vp, vp, sz, sz, u32p, f64p, C.c_uint32, C.c_int64, u32p, C.POINTER(sz)]),
         "vmb_host_alloc": (vp, [sz]),
         "vmb_host_free": (None, [vp]),
         "vmb_ctx_last_stage_ms": (C.c_float, [vp, C.c_int]),

@@ -1884,6 +1884,7 @@ extern "C" int vmb_eval_rollup_aggr_device(vmb_ctx* ctx, const vmb_blocks* b, in
 #include "transform.inc"
 #include "range_transform.inc"
 #include "histogram.inc"
+#include "vmrange.inc"
 
 // ------------------------------------------------------------------------------------------------ batched host encoder
 #include <atomic>

@@ -3,6 +3,9 @@
 Names follow the reference (rollup.go / eval.go / aggr_incremental.go); every compute call goes to libvmb200.
 """
 import ctypes as C
+import math
+import re
+import string
 
 import numpy as np
 
@@ -604,7 +607,133 @@ def histogram(name, vals_dev_ptr, nrows, points, group_ids, les, ngroups, out_de
     return flags[:nout].astype(bool)
 
 
-MATRIX_AGGR_FUNCS = {n: i for i, n in enumerate(
+_GO_SPECIAL = re.compile(r"[+-]?(inf|infinity)|nan", re.I)
+_GO_DEC = re.compile(r"[+-]?([0-9_]+\.?[0-9_]*|\.[0-9_]+)([eE][+-]?[0-9][0-9_]*)?")
+_GO_HEX = re.compile(r"[+-]?0[xX]([0-9a-fA-F_]+\.?[0-9a-fA-F_]*|\.[0-9a-fA-F_]+)[pP][+-]?[0-9][0-9_]*")
+
+
+def _go_underscores_ok(s):
+    """underscores only between digits, or between the base prefix and a digit, as in Go's number literals"""
+    s = s[1:] if s[:1] in "+-" else s
+    saw, i, hexa = "^", 0, False
+    if len(s) >= 2 and s[0] == "0" and s[1] in "xX":
+        saw, i, hexa = "0", 2, True
+    for c in s[i:]:
+        if c.isdigit() or (hexa and c in "abcdefABCDEF"):
+            saw = "0"
+        elif c == "_":
+            if saw != "0":
+                return False
+            saw = "_"
+        elif saw == "_":
+            return False
+        else:
+            saw = "!"
+    return saw != "_"
+
+
+def go_parse_float(s):
+    """strconv.ParseFloat(s, 64) -> the float, or None where Go returns an error.  Go's strconv source is not part of the
+    reference, so this restates Go's published documentation of ParseFloat: decimal and hexadecimal floating-point numbers in
+    the syntax of Go's floating-point literals (a hexadecimal one needs its p exponent; underscores may separate digits, as
+    in Go literals), rounded to nearest even; "NaN", and "Inf" / "Infinity" with an optional sign, in any case; nothing
+    around the number (no spaces).  A number beyond the float64 range is ErrRange (None); one below it rounds to 0."""
+    if _GO_SPECIAL.fullmatch(s):
+        low = s.lower()
+        return float("nan") if low == "nan" else float("-inf") if low[0] == "-" else float("inf")
+    hexa = _GO_HEX.fullmatch(s) or None
+    m = hexa or _GO_DEC.fullmatch(s)
+    if not m or not any(c in string.hexdigits if hexa else c.isdigit() for c in m.group(1)):  # a mantissa digit
+        return None
+    if "_" in s and not _go_underscores_ok(s):
+        return None
+    t = s.replace("_", "")
+    try:
+        v = float.fromhex(t) if hexa else float(t)
+    except (OverflowError, ValueError):
+        return None
+    return None if math.isinf(v) else v
+
+
+VR_KEEP = 0xFFFFFFFE  # VMB_VR_KEEP
+VR_KINDS = ["kept", "bucket", "gap", "+Inf"]  # enum vmb_vr_kind
+
+
+def prometheus_buckets(vals_dev_ptr, nrows, points, vmranges, has_le, group_ids, device_alloc, ctx=None):
+    """prometheus_buckets (vmrangeBucketsToLE, transform.go:494, vmb_vmrange_to_le) on a DEVICE matrix [nrows x points].
+    vmranges: every row's `vmrange` label, None (or "") where it has none; has_le: whether the row has a non-empty `le`;
+    group_ids: the dense id of every row's label set without `vmrange` and `le` (read for rows with a valid vmrange).
+    device_alloc(nbytes) -> object with .ptr.  -> (out, n, src, kinds, les): out holds [n x points] (sized by a first call that
+    only counts); per output row: src, the input row it comes from (a gap or +Inf row takes its labels); kinds, an index into
+    VR_KINDS; les, its `le` string (None for a kept row, which keeps its own `le`)."""
+    ctx = ctx or _lib.default_context()
+    n = int(nrows)
+    if len(vmranges) != n or len(has_le) != n or len(group_ids) != n:
+        raise ValueError("prometheus_buckets: need one vmrange, has_le and group id per row (%d rows)" % n)
+    gids = np.full(n, 0xFFFFFFFF, dtype=np.uint32)
+    starts, ends = np.zeros(n), np.zeros(n)
+    skeys, ekeys = np.zeros(n, dtype=np.uint32), np.zeros(n, dtype=np.uint32)
+    strings, ids = [], {}
+
+    def key(s):
+        if s not in ids:
+            ids[s] = len(strings)
+            strings.append(s)
+        return ids[s]
+    for i, vr in enumerate(vmranges):
+        if not vr:
+            if has_le[i]:
+                gids[i] = VR_KEEP
+            continue
+        k = vr.find("...")
+        if k < 0:
+            continue
+        a, b = vr[:k], vr[k + 3:]
+        fa, fb = go_parse_float(a), go_parse_float(b)
+        if fa is None or fb is None:
+            continue
+        gids[i], starts[i], ends[i], skeys[i], ekeys[i] = int(group_ids[i]), fa, fb, key(a), key(b)
+    grouped = gids[gids < VR_KEEP]
+    ngroups = int(grouped.max()) + 1 if grouped.size else 0
+    nout = C.c_size_t(0)
+    src, kind, le = (np.zeros(1, dtype=np.uint32), np.zeros(1, dtype=np.uint8), np.zeros(1, dtype=np.uint32))
+    u32 = lambda a: a.ctypes.data_as(_lib.u32p)
+    f64 = lambda a: a.ctypes.data_as(_lib.f64p)
+
+    def call(out_ptr):
+        return lib().vmb_vmrange_to_le(ctx.h, C.c_void_p(int(vals_dev_ptr)), n, int(points), u32(gids), f64(starts), f64(ends),
+                                       u32(skeys), u32(ekeys), ngroups, out_ptr, C.byref(nout), u32(src),
+                                       kind.ctypes.data_as(_lib.u8p), u32(le))
+    check(call(None), allow=(-54,))  # VMB_ERR_CAP: the count
+    rows = nout.value
+    src, kind, le = (np.zeros(max(rows, 1), dtype=np.uint32), np.zeros(max(rows, 1), dtype=np.uint8),
+                     np.zeros(max(rows, 1), dtype=np.uint32))
+    out = device_alloc(max(rows * int(points) * 8, 8))
+    if rows:
+        check(call(C.c_void_p(int(out.ptr))))
+    les = [None if k == 0 else "+Inf" if k == 3 else strings[x] for k, x in zip(kind[:rows].tolist(), le[:rows].tolist())]
+    return out, rows, src[:rows].astype(np.int64), kind[:rows].copy(), les
+
+
+def buckets_limit(limit, vals_dev_ptr, nrows, points, group_ids, les, ngroups, ctx=None):
+    """buckets_limit(limit, buckets) (transform.go:386, vmb_buckets_limit) on a DEVICE `le` matrix [nrows x points], usually
+    the output of prometheus_buckets.  group_ids: the dense id of every row's label set without `le`, 0xffffffff for a row
+    without a parsable `le`; les: every row's parsed `le`.  -> the rows kept, in output order (np.int64); the matrix is not
+    changed."""
+    ctx = ctx or _lib.default_context()
+    g = np.ascontiguousarray(group_ids, dtype=np.uint32)
+    le = np.ascontiguousarray(les, dtype=np.float64)
+    if g.size != int(nrows) or le.size != int(nrows):
+        raise ValueError("buckets_limit: need one group id and one le per row (%d rows)" % nrows)
+    rows = np.zeros(max(int(nrows), 1), dtype=np.uint32)
+    nout = C.c_size_t(rows.size)
+    check(lib().vmb_buckets_limit(ctx.h, C.c_void_p(int(vals_dev_ptr)), int(nrows), int(points), g.ctypes.data_as(_lib.u32p),
+                                  le.ctypes.data_as(_lib.f64p), int(ngroups), int(limit), rows.ctypes.data_as(_lib.u32p),
+                                  C.byref(nout)))
+    return rows[:nout.value].astype(np.int64)
+
+
+MATRIX_AGGR_FUNCS ={n: i for i, n in enumerate(
     ["sum", "sum2", "min", "max", "avg", "count", "group", "geomean", "stddev", "stdvar", "share", "zscore"])}
 
 
