@@ -15,6 +15,12 @@
  *     VMB_ERR_CUDA if no sm_90 (H100-class) device is usable.
  *   - all kernels of one vmb_ctx are issued on the ctx's stream (vmb_ctx_set_stream), so the caller can
  *     bracket them with its own CUDA events.
+ *   - an entry point with a host output returns with it written and the ctx's stream drained (pinned or pageable).
+ *     These return before their kernels finish (wait on the ctx's stream before reading their device outputs):
+ *       vmb_group_first_value, vmb_topk_candidates   -- their kernels read the ctx's group scratch (grp)
+ *       vmb_topk_merge, vmb_aggr_merge, vmb_aggr_prepare_allreduce, vmb_series_from_matrix -- no ctx scratch
+ *       vmb_binary_op without row lists, vmb_transform without per-point arguments         -- no ctx scratch
+ *     Growing that scratch in a later call frees it with cudaFree, which waits for the device first.
  */
 #ifndef VMB200_H
 #define VMB200_H

@@ -1110,7 +1110,8 @@ extern "C" int vmb_unmarshal_int64(vmb_ctx* ctx, int64_t* dst, size_t n, const u
     if (rc == VMB_OK || rc == VMB_ERR_BLOCK_FAILED) {
         if (status) rc = status;
         else {
-            cudaError_t e = cudaMemcpy(dst, s->d_vals, n * 8, cudaMemcpyDeviceToHost);
+            cudaError_t e = cudaMemcpyAsync(dst, s->d_vals, n * 8, cudaMemcpyDeviceToHost, ctx->stream);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);  // dst may be pinned: the copy lands before return
             rc = e == cudaSuccess ? VMB_OK : VMB_ERR_CUDA;
         }
     }
@@ -1772,7 +1773,8 @@ static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t
     if (*h_bail) {
         const size_t n0 = sub.size();
         sub.resize(n0 + *h_bail);
-        CU(cudaMemcpy(sub.data() + n0, d_bail_list, (size_t)*h_bail * 4, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpyAsync(sub.data() + n0, d_bail_list, (size_t)*h_bail * 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
         std::sort(sub.begin(), sub.end());
     }
     if (ctx->timing) {
