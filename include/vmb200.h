@@ -518,6 +518,40 @@ int vmb_vmrange_to_le(vmb_ctx* ctx, const double* d_buckets, size_t nrows, size_
  * Errors as vmb_vmrange_to_le. */
 int vmb_buckets_limit(vmb_ctx* ctx, const double* d_buckets, size_t nrows, size_t points, const uint32_t* group_ids,
                       const double* les, uint32_t ngroups, int64_t limit, uint32_t* out_rows, size_t* nout);
+/* The aggregates that rank whole series, on a DEVICE matrix d_vals [nseries x P]: topk_min / topk_max / topk_avg / topk_median /
+ * topk_last(k, q [, "remaining_sum"]) by (...) and their bottomk_* twins (reverse != 0) (newAggrFuncRangeTopK aggr.go:677 ->
+ * getRangeTopKTimeseries :704), and outliersk(k, q) by (...) (aggrFuncOutliersK :1040; reverse must be 0, d_remaining NULL).
+ * group_ids: HOST, dense ids < ngroups.  Rows without a non-NaN value belong to no group (removeEmptySeries :124).  ks: HOST, one k
+ * per point (getScalar); kn = getIntK(ks[p], n_g) (:793: NaN and negative are 0, truncation, at most the n_g rows of the group).
+ *   score  MIN / MAX (:804, :818): the first value while that is NaN, then the smaller / larger non-NaN ones; AVG (:832): the sum of
+ *          the non-NaN values in point order over their number; MEDIAN (:848): quantile(0.5) of the non-NaN values; LAST (:852): the
+ *          last non-NaN value; OUTLIERSK (:1053): the sum over the points, in order and without FMA, of (v - median)^2, the median
+ *          (:1066) taken per point over the group's rows -- a row with a NaN anywhere scores NaN.
+ *   order  every group is ordered as a STABLE sort of its rows, in ascending row order, by lessWithNaNs (:1259; reverse:
+ *          greaterWithNaNs :1270; a NaN score is the worst in both).  Both are strict weak orders, so this is what Go's sort.Slice
+ *          returns for up to 12 rows (its insertion sort) and one of the outcomes of its unstable pdqsort beyond that; rows with
+ *          distinct non-NaN scores are not affected.  -0.0 and +0.0 tie.
+ *   mask   at point p every row but the kn best of its group becomes NaN (fillNaNsAtIdx :786).  A survivor is a row that then still
+ *          holds a non-NaN value.  ONLY SURVIVORS ARE WRITTEN: every other row of d_vals -- one without a value, one outside the k
+ *          best of every point, one that holds no value where it is among them -- keeps the bits it had, and is not in out_rows.
+ *   d_remaining: DEVICE [ngroups x P] or NULL (no third argument): per (group, point) 0 + v + v ... over the non-NaN values of the
+ *          rows outside the kn best, from the worst on, NaN for none (getRemainingSumTimeseries :751).  remaining_nonempty: HOST,
+ *          ngroups bytes, required with d_remaining: 1 where the group's row holds a value.
+ *   row_nonempty: HOST, nseries bytes, 1 where the row held a non-NaN value before the call (as in vmb_aggr_matrix: the host derives
+ *          from it which groups exist and `limit N`).
+ *   out_rows: HOST, capacity nseries: the survivors, groups in ascending id, each from best to worst (the reference's output order
+ *          after reverseSeries :743).  out_counts: HOST, ngroups: the survivors of every group.  The host puts a group's
+ *          remaining-sum row, where it holds a value, before the group's survivors, applies `limit N` and owns the labels.
+ *   scores: HOST, nseries doubles, or NULL: the score of every row (one without a value: NaN).
+ * Bit-exact except the sign of a zero MEDIAN score where a tied rank holds both -0.0 and +0.0 (the reference's sort is not stable
+ * there either; the order of the rows does not depend on it).  VMB_ERR_INVALID_ARG for an unknown func, ngroups == 0, a group id
+ * >= ngroups, a missing pointer, reverse or d_remaining with OUTLIERSK, or nseries / points > 2^31 - 1; VMB_ERR_NOMEM when the
+ * scratch (MEDIAN: at most 2 GiB of keys, as vmb_transform_range) cannot be had; d_vals, d_remaining and the host outputs are
+ * untouched in both cases.  nseries == 0 or points == 0: out_counts is zeroed, nothing else. */
+enum vmb_rank_func { VMB_RK_MIN = 0, VMB_RK_MAX, VMB_RK_AVG, VMB_RK_MEDIAN, VMB_RK_LAST, VMB_RK_OUTLIERSK };
+int vmb_aggr_rank(vmb_ctx* ctx, int func, int reverse, double* d_vals, size_t nseries, size_t points, const uint32_t* group_ids,
+                  uint32_t ngroups, const double* ks, double* d_remaining, unsigned char* remaining_nonempty,
+                  unsigned char* row_nonempty, uint32_t* out_rows, uint32_t* out_counts, double* scores);
 
 /* ---- multi-GPU: one process per GPU, the ONE exchange step of the path inside the library (SURVEY 8e) ------------------
  * aggr(rollup(m[d])) by (...): every rank folds its shard of the series into {values, counts}[G x P] (the per-worker

@@ -1887,6 +1887,7 @@ extern "C" int vmb_eval_rollup_aggr_device(vmb_ctx* ctx, const vmb_blocks* b, in
 #include "range_transform.inc"
 #include "histogram.inc"
 #include "vmrange.inc"
+#include "rank_aggr.inc"
 
 // ------------------------------------------------------------------------------------------------ batched host encoder
 #include <atomic>

@@ -791,6 +791,49 @@ def aggr_order(name, vals_dev_ptr, nseries, points, out_dev_ptr=None, group_ids=
     return groups
 
 
+RANK_FUNCS = {n: i for i, n in enumerate(["min", "max", "avg", "median", "last", "outliersk"])}
+RANK_AGGR_NAMES = ["%s_%s" % (t, s) for t in ("topk", "bottomk") for s in ("min", "max", "avg", "median", "last")] + ["outliersk"]
+
+
+def aggr_rank(name, ks, vals_dev_ptr, nseries, points, group_ids=None, ngroups=1, remaining_dev_ptr=None, limit=0, ctx=None):
+    """topk_min / topk_max / topk_avg / topk_median / topk_last(k, q [, "remaining_sum"]) by (...) [limit N], their bottomk_* twins
+    (getRangeTopKTimeseries aggr.go:704) and outliersk(k, q) (:1040) on a DEVICE matrix [nseries x points] (vmb_aggr_rank).  ks: a
+    number or one k per point.  The surviving rows are masked in place (NaN where a row is not among the point's k best of its
+    group); every other row stays as it was.  remaining_dev_ptr: [ngroups x points] for the remaining-sum rows (the third argument;
+    not for outliersk).  -> (out, scores): out (np.int64) lists the reference's output, groups in order of their first non-empty
+    row and cut at `limit` (0 = no limit), per group -(g + 1) for the remaining-sum row of group g where it holds a value, then
+    the surviving rows from best to worst; scores: every row's score."""
+    ctx = ctx or _lib.default_context()
+    name = name.lower()
+    if name not in RANK_AGGR_NAMES:
+        raise ValueError("aggr_rank: unknown function %r" % name)
+    g = np.zeros(nseries, dtype=np.uint32) if group_ids is None else np.ascontiguousarray(group_ids, dtype=np.uint32)
+    k = np.ascontiguousarray(np.broadcast_to(np.asarray(ks, dtype=np.float64), (points,)))
+    rem_ne = np.zeros(max(int(ngroups), 1), dtype=np.uint8)
+    nonempty = np.zeros(max(nseries, 1), dtype=np.uint8)
+    rows = np.zeros(max(nseries, 1), dtype=np.uint32)
+    counts = np.zeros(max(int(ngroups), 1), dtype=np.uint32)
+    scores = np.full(max(nseries, 1), np.nan)
+    u8 = lambda a: a.ctypes.data_as(_lib.u8p)
+    u32 = lambda a: a.ctypes.data_as(_lib.u32p)
+    check(lib().vmb_aggr_rank(ctx.h, RANK_FUNCS[name.split("_")[-1]], int(name.startswith("bottomk_")), C.c_void_p(int(vals_dev_ptr)),
+                              int(nseries), int(points), u32(g), int(ngroups), k.ctypes.data_as(_lib.f64p),
+                              C.c_void_p(int(remaining_dev_ptr or 0)), u8(rem_ne) if remaining_dev_ptr else None, u8(nonempty),
+                              u32(rows), u32(counts), scores.ctypes.data_as(_lib.f64p)))
+    ne = nonempty[:nseries].astype(bool)
+    _, first = np.unique(g[ne], return_index=True)  # aggrPrepareSeries aggr.go:139: groups in order of first non-empty row
+    groups = g[ne][np.sort(first)]
+    if limit > 0:
+        groups = groups[:limit]
+    starts = np.concatenate([[0], np.cumsum(counts[:ngroups], dtype=np.int64)])
+    out = []
+    for gid in groups.tolist():
+        if rem_ne[gid]:
+            out.append(-(gid + 1))
+        out.extend(rows[starts[gid]:starts[gid + 1]].tolist())
+    return np.array(out, dtype=np.int64), scores[:nseries]
+
+
 def aggr_quantile(phis, vals_dev_ptr, nseries, points, out_dev_ptr, group_ids=None, ngroups=1, ctx=None):
     """quantile(phi, q) by (...) / median (phi = 0.5)  aggr.go:1217 on a DEVICE matrix -> out_dev_ptr [ngroups x points]"""
     ctx = ctx or _lib.default_context()
