@@ -45,6 +45,41 @@
 #define FU_STAGE (16 + FU_FILL + 16)      /* 16 bytes of the previous tile in front, 16 bytes of padding behind */
 #define FU_MAX_EVENTS 32                  /* counter resets inside one fill handled by the parallel path */
 
+// Phase-clock build (-DVMB_FUSED_PHASES, scripts/exp_fused_phases.py; never the product): lane 0 of every warp adds the clock64()
+// cycles since its previous mark to the phase that just ended, and the CTA's totals land in fu_phase_cyc[blockIdx.x].  Without
+// the macro FU_PH() expands to nothing and the kernel compiles to the same SASS.
+enum {
+    FU_PH_SETUP,   // series setup, the first copy of a series, the tail of a series
+    FU_PH_TERM,    // terminator scan and the tile counts
+    FU_PH_PARSE,   // varint parse (and generated rows of constant columns)
+    FU_PH_SCAN,    // the two sum scans over the warp and over the warps
+    FU_PH_EMIT,    // replay of the values and float conversion
+    FU_PH_RCR,     // counter-reset work
+    FU_PH_POINTS,  // points and the slide of the resident rows
+    FU_PH_WAIT,    // barriers, and copies of fills after a series' first
+    FU_PH_N,
+    FU_PH_FILLS = FU_PH_N,  // counters kept by warp 0: fills, series
+    FU_PH_SERIES,
+    FU_PH_SLOTS
+};
+#ifdef VMB_FUSED_PHASES
+#define FU_PH_CTAS (VMB_SMS * FU_CTAS_PER_SM)
+__device__ unsigned long long fu_phase_cyc[FU_PH_CTAS][FU_PH_SLOTS];
+#define FU_PH(k)                                              \
+    do {                                                      \
+        const long long ph_c = clock64();                     \
+        if (lane == 0) S.ph[w][(k)] += (unsigned long long)(ph_c - ph_t); \
+        ph_t = ph_c;                                          \
+    } while (0)
+#define FU_PH_COUNT(k) \
+    do {               \
+        if (tid == 0) S.ph[0][(k)]++; \
+    } while (0)
+#else
+#define FU_PH(k) ((void)0)
+#define FU_PH_COUNT(k) ((void)0)
+#endif
+
 struct FusedParams {
     const vmb_block_desc* descs;
     const ColInfo* cols;
@@ -103,6 +138,9 @@ struct FusedSmem {
     unsigned long long s_thr[FU_THREADS];  // this thread's share of samplesScanned over the series the CTA finished
     unsigned long long s_ser[FU_THREADS];  // the same for the current series (dropped when it is handed to the un-fused path)
     FuSeries ser;  // the current series (read where it is used: it stays valid for the whole series)
+#ifdef VMB_FUSED_PHASES
+    unsigned long long ph[FU_WARPS][FU_PH_SLOTS];
+#endif
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -418,6 +456,10 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
         mbar_init(&S.mbar[1], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+#ifdef VMB_FUSED_PHASES
+    for (uint32_t k = tid; k < FU_WARPS * FU_PH_SLOTS; k += FU_THREADS) (&S.ph[0][0])[k] = 0;
+    long long ph_t = clock64();
+#endif
     __syncthreads();
 
     for (uint32_t li = blockIdx.x; li < P.nlist; li += gridDim.x) {
@@ -462,6 +504,8 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
         S.s_ser[tid] = tid == 0 ? n : 0u;  // samplesScanned starts at len(values) rollup.go:766
         __syncthreads();
         if (!bail) prev_raw = S.val[0];
+        FU_PH_COUNT(FU_PH_SERIES);
+        FU_PH(FU_PH_SETUP);
 
         uint32_t guard = 0;
         while (!bail && (p < P.npoints || !stream_done)) {
@@ -473,11 +517,14 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
             uint32_t cnt_old = cnt;
             bool progressed = false;
             if (is_stream && !stream_done) {
+                FU_PH(FU_PH_POINTS);
+                FU_PH_COUNT(FU_PH_FILLS);
                 if (copy_pending) {
                     mbar_wait(&S.mbar[buf], (par >> buf) & 1u);
                     par ^= 1u << buf;
                     copy_pending = false;
                 }
+                FU_PH(fs ? FU_PH_WAIT : FU_PH_SETUP);
                 const uint8_t* st = &S.stage[buf][16];  // aligned stream byte `fs` sits at st[0]
                 const uint32_t end_al = SE.end_al;
                 const int64_t vlo = (int64_t)SE.shift, vhi = vlo + SE.len;  // valid stream positions in aligned coordinates
@@ -522,7 +569,9 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                 }
                 if (lane == 31) S.w_cnt[w] = incl;
                 if (tid == 0) S.nev = 0;  // (everybody read the previous fill's events before the barrier that ended it)
+                FU_PH(FU_PH_TERM);
                 __syncthreads();
+                FU_PH(FU_PH_WAIT);
                 // whole tiles that fit the resident rows (pass-through once the points are done: rows are only validated)
                 const bool discard = p >= P.npoints;
                 if (discard) { cnt = 1; cnt_old = 1; }  // rows are not needed any more: decode over the same ring slots
@@ -551,6 +600,7 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                         issue_copy(fs_next, buf ^ 1u);
                         copy_pending = true;
                     }
+                    FU_PH(FU_PH_TERM);
                     // ---- parse: the varints whose terminator lies in this lane's 16 bytes
                     uint64_t s1 = 0, s2 = 0;
                     const uint32_t row0 = base + cnt + rb + incl - cl;  // absolute row of the lane's first value
@@ -667,6 +717,7 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                                         off + 16u * g);
                         }
                     }
+                    FU_PH(FU_PH_PARSE);
                     // ---- scan (s1, s2) over the warp.  combine(A then B): s2 = s2A + s2B + cntB * s1A, so with E1(l) = the plain
                     // exclusive prefix of s1, the inclusive prefix of s2 is the plain prefix sum of t_l = s2_l + cnt_l * E1(l): two sum
                     // scans (wrapping int64 arithmetic: bit-identical to the sequential Go loop), the counts are known from step 1
@@ -692,7 +743,9 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                         S.w_s2[w] = is2;
                     }
                     if (bad) S.flags = 1u;
+                    FU_PH(FU_PH_SCAN);
                     __syncthreads();
+                    FU_PH(FU_PH_WAIT);
                     if (S.flags & 1u) bail = true;
                     // exclusive prefix over the warps in front, and the totals of the fill: lane k < K holds warp k's triple, one
                     // FU_WARPS-lane scan, warp w picks lane w - 1 (prefix) and everybody lane K - 1 (totals)
@@ -730,6 +783,7 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                         ts1 = shfl_u64(a1, src_t);
                         ts2 = shfl_u64(a2, src_t);
                     }
+                    FU_PH(FU_PH_SCAN);
                     // ---- emit: replay the lane's values with the scanned prefix, mantissa -> float64 in place
                     const uint32_t ecnt = incl - cl;         // lanes in front, this warp (step 1)
                     const uint64_t es1 = es1_, es2 = is2 - t2;
@@ -742,43 +796,68 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                         uint64_t d1 = D1 + fs1;
                         uint64_t v = delta2 ? (V + fs2 + (uint64_t)fcnt * D1) : (V + fs1);
                         bool saw_stale = false;
+                        uint32_t cand = 0;  // bit k: row0 + k holds a smaller value than the row in front (a lane has <= 32 rows)
+                        const uint64_t v0 = v;
                         const Dec dec = fu_dec(SE);
                         auto emit_run = [&](auto is_delta2) {
                             constexpr bool D2 = decltype(is_delta2)::value;
-                            for (uint32_t k = 0; k < cl; k++) {
-                                const uint64_t pv = v;
-                                const uint64_t x = (uint64_t)fu_lds_i64(val_s, row0 + k);
-                                if (D2) {
-                                    d1 += x;
-                                    v += d1;
-                                } else {
-                                    v += x;
-                                }
-                                double f = dec.conv_plain((int64_t)v);
-                                if ((uint64_t)v - 0x7FFFFFFFFFFFFFFEull < 3ull) {  // vStaleNaN / vInfPos / vInfNeg (decimal.go:403-417)
-                                    f = dec.conv((int64_t)v);
-                                    saw_stale |= ((int64_t)v == VMB_V_STALE_NAN);
-                                }
-                                if (do_rcr && (int64_t)v < (int64_t)pv) {
-                                    // candidate counter reset (the conversion is monotone): the exact test is on the floats, rollup.go:928
-                                    const double pf = dec.conv((int64_t)pv);
-                                    const double dd = f - pf;
-                                    if (dd < 0) {
-                                        const double amt = ((-dd * 8) < pf) ? (pf - f) : pf;
-                                        const uint32_t e = atomicAdd(&S.nev, 1u);
-                                        if (e < FU_MAX_EVENTS) {
-                                            S.ev_row[e] = row0 + k;
-                                            S.ev_amt[e] = amt;
+                            // four rows per step: their deltas are loaded first, their conversions are independent of each other and
+                            // overlap, their stores come last (row by row, every row waited for its load and for the store in front)
+                            for (uint32_t k = 0; k < cl; k += 4) {
+                                uint64_t x[4], vv[4];
+#pragma unroll
+                                for (int i = 0; i < 4; i++) x[i] = (uint64_t)fu_lds_i64(val_s, row0 + k + i);  // (past cl: not used)
+#pragma unroll
+                                for (int i = 0; i < 4; i++) {
+                                    const uint64_t pv = v;
+                                    if (k + i < cl) {
+                                        if (D2) {
+                                            d1 += x[i];
+                                            v += d1;
+                                        } else {
+                                            v += x[i];
                                         }
+                                        cand |= (uint32_t)((int64_t)v < (int64_t)pv) << (k + i);
+                                    }
+                                    vv[i] = v;
+                                }
+                                double f[4];
+#pragma unroll
+                                for (int i = 0; i < 4; i++) f[i] = dec.conv_plain((int64_t)vv[i]);
+#pragma unroll
+                                for (int i = 0; i < 4; i++) {
+                                    if (k + i < cl) {
+                                        if (vv[i] - 0x7FFFFFFFFFFFFFFEull < 3ull) {  // vStaleNaN / vInfPos / vInfNeg (decimal.go:403-417)
+                                            f[i] = dec.conv((int64_t)vv[i]);
+                                            saw_stale |= ((int64_t)vv[i] == VMB_V_STALE_NAN);
+                                        }
+                                        fu_sts(val_s, row0 + k + i, f[i]);
                                     }
                                 }
-                                fu_sts(val_s, row0 + k, f);
                             }
                         };
                         if (delta2) emit_run(std::true_type{});
                         else emit_run(std::false_type{});
+                        // candidate counter resets (the conversion is monotone): the exact test is on the floats, rollup.go:928
+                        if (do_rcr && cand) {
+                            do {
+                                const uint32_t k = (uint32_t)__ffs((int)cand) - 1u;
+                                cand &= cand - 1u;
+                                const double f = fu_lds(val_s, row0 + k), pf = k ? fu_lds(val_s, row0 + k - 1u) : dec.conv((int64_t)v0);
+                                const double dd = f - pf;
+                                if (dd < 0) {
+                                    const double amt = ((-dd * 8) < pf) ? (pf - f) : pf;
+                                    const uint32_t e = atomicAdd(&S.nev, 1u);
+                                    if (e < FU_MAX_EVENTS) {
+                                        S.ev_row[e] = row0 + k;
+                                        S.ev_amt[e] = amt;
+                                    }
+                                }
+                            } while (cand);
+                        }
                         if (saw_stale && stale_matters) S.flags_emit = 1u;
                     }
+                    FU_PH(FU_PH_EMIT);
                     // ---- carries: thread 0 stores them behind the barrier that ends the fill (every lane has read the old ones by then)
                     uint64_t nV = 0, nD1 = 0;
                     if (tid == 0) {
@@ -802,6 +881,7 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                         if (N != nvar) bail = true;
                     }
                     __syncthreads();
+                    FU_PH(FU_PH_WAIT);
                     if (tid == 0) {
                         S.nd_v = nV;
                         S.nd_d1 = nD1;
@@ -825,7 +905,9 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                 gen_rows += take;
                 cnt += take;
                 N = gen_rows - 1;
+                FU_PH(FU_PH_PARSE);
                 __syncthreads();
+                FU_PH(FU_PH_WAIT);
                 if (S.flags & 1u) bail = true;
             }
             if (bail) break;
@@ -841,8 +923,18 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                 } else if (nev == 0 && corr != 0.0 && isfinite(corr) && fu_ld(S.val, base + cnt_old) + corr >= fu_ld(S.val, base + cnt_old - 1)) {
                     // no value drop inside the fill (nor at its front) and its first corrected row is not below the last output: raw
                     // rows are non-decreasing, x -> RN(x + corr) keeps the order, so the clamp of rollup.go:954 cannot fire: one pass
-                    for (uint32_t k = cnt_old + tid; k < cnt; k += FU_THREADS) fu_sts(val_s, base + k, fu_lds(val_s, base + k) + corr);
+                    // (four rows per thread and step, their loads issued before the first store)
+                    for (uint32_t k = cnt_old + tid; k < cnt; k += 4 * FU_THREADS) {
+                        double x[4];
+#pragma unroll
+                        for (int i = 0; i < 4; i++) x[i] = fu_lds(val_s, base + k + i * FU_THREADS);  // (past cnt: values not used)
+#pragma unroll
+                        for (int i = 0; i < 4; i++)
+                            if (k + i * FU_THREADS < cnt) fu_sts(val_s, base + k + i * FU_THREADS, x[i] + corr);
+                    }
+                    FU_PH(FU_PH_RCR);
                     __syncthreads();
+                    FU_PH(FU_PH_WAIT);
                 } else if (nev || corr != 0.0) {
                     if (tid == 0) {
                         // events in row order, corrections accumulated sequentially like the Go loop
@@ -864,7 +956,9 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                             S.ev_cum[a] = c;
                         }
                     }
+                    FU_PH(FU_PH_RCR);
                     __syncthreads();
+                    FU_PH(FU_PH_WAIT);
                     // corrected values are non-decreasing unless float rounding interferes: check that first, without writing
                     const double prev_out = RV[base + cnt_old - 1];
                     bool viol = false;
@@ -879,7 +973,9 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                         const double mp = k == cnt_old ? prev_out : RV[ar - 1] + cp;
                         viol |= !(mk >= mp);  // a clamp would fire, or a NaN is involved
                     }
+                    FU_PH(FU_PH_RCR);
                     const int any_viol = __syncthreads_or((int)viol);
+                    FU_PH(FU_PH_WAIT);
                     if (!any_viol) {
                         for (uint32_t k = cnt_old + tid; k < cnt; k += FU_THREADS) {
                             const uint32_t ar = base + k;
@@ -902,10 +998,13 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                         }
                     }
                     if (nev) corr = S.ev_cum[nev - 1];
+                    FU_PH(FU_PH_RCR);
                     __syncthreads();
+                    FU_PH(FU_PH_WAIT);
                 }
                 prev_raw = raw_last;
             }
+            FU_PH(FU_PH_RCR);
 
             // ================= points whose window lies inside the resident rows
             const int32_t start_r = SE.start_r, step32 = SE.step32, win32 = SE.win32, mpi32 = SE.mpi32;
@@ -920,7 +1019,9 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
             }
             if (p_end <= p) {
                 if (!progressed) bail = true;  // the window of point p does not fit FU_CAP rows: un-fused path
+                FU_PH(FU_PH_POINTS);
                 __syncthreads();
+                FU_PH(FU_PH_WAIT);
                 continue;
             }
             {
@@ -939,32 +1040,8 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                 auto put = [&](uint32_t q, double v) { out_row[q] = v; };
                 uint32_t sc_interior = spc ? spc : (uint32_t)rate_rows;  // samplesScanned of an interior rate() point
                 asm volatile("" : "+r"(sc_interior));
-#pragma unroll 2
-                for (uint32_t q = p + tid; q < p_end; q += FU_THREADS) {
-                    if ((F == VMB_RF_RATE || F == VMB_RF_DELTA) && lin && rate_dt > 0 && prev_always) {
-                        // interior point: the window [i, j) holds rate_rows rows and row i - 1 exists: (v[j-1] - v[i-1]) / D
-                        const int32_t is_ = iq0 + (int32_t)q * lin_k;
-                        if (is_ >= 1 && is_ + rate_rows <= (int32_t)n) {
-                            const double vp = fu_lds(val_s, (uint32_t)is_ - 1u), vl = fu_lds(val_s, (uint32_t)(is_ + rate_rows) - 1u);
-                            const double x = vl - vp;
-                            if (F == VMB_RF_DELTA) {  // rollupDelta rollup.go:1859 with a previous value: values[n - 1] - prevValue
-                                if (!isnan(vp)) {
-                                    sc32 += sc_interior;
-                                    put(q, x);
-                                    continue;
-                                }
-                            } else {
-                                const uint32_t ex = ((uint32_t)__double2hiint(x) >> 20) & 0x7ffu;
-                                if (!isnan(vp) && (x == 0.0 || ex - 123u < 1800u)) {
-                                    const double q0 = __dmul_rn(x, rate_R);
-                                    const double rem = __fma_rn(-q0, rate_D, x);
-                                    sc32 += sc_interior;
-                                    put(q, x == 0.0 ? x : __fma_rn(rem, rate_R, q0));
-                                    continue;
-                                }
-                            }
-                        }
-                    }
+                // a point from its window edges (rate_edges / window_point): every point the interior path below does not take
+                auto point = [&](uint32_t q) {
                     const int32_t xj = start_r + (int32_t)q * step32;
                     uint32_t i, j;
                     if (lin) {  // edges advance by a whole number of rows per point: no division
@@ -1001,11 +1078,58 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                         const int64_t t_im1 = SE.t_org + ((int64_t)i - 1) * SE.dts;
                         put(q, window_point<F>(rc, FuVals{S.val, i}, FuTs{t_im1 + SE.dts, SE.dts}, i, n, i, j, q, SE.window, SE.max_prev, scanned));
                     }
+                };
+                if ((F == VMB_RF_RATE || F == VMB_RF_DELTA) && lin && rate_dt > 0 && prev_always) {
+                    // interior points: the window [i, j) holds rate_rows rows and row i - 1 exists: (v[j-1] - v[i-1]) / D.  Four points
+                    // per thread, their eight edge loads issued before any arithmetic (a point off the range reads ring slots whose
+                    // values are not used)
+                    for (uint32_t q = p + tid; q < p_end; q += 4 * FU_THREADS) {
+                        double vp[4], vl[4];
+#pragma unroll
+                        for (int k = 0; k < 4; k++) {
+                            const int32_t is_ = iq0 + (int32_t)(q + k * FU_THREADS) * lin_k;
+                            vp[k] = fu_lds(val_s, (uint32_t)is_ - 1u);
+                            vl[k] = fu_lds(val_s, (uint32_t)(is_ + rate_rows) - 1u);
+                        }
+                        uint32_t rest = 0;  // points of the four the interior path does not take
+#pragma unroll
+                        for (int k = 0; k < 4; k++) {
+                            const uint32_t qk = q + k * FU_THREADS;
+                            if (qk >= p_end) break;
+                            const int32_t is_ = iq0 + (int32_t)qk * lin_k;
+                            const double x = vl[k] - vp[k];
+                            bool ok = is_ >= 1 && is_ + rate_rows <= (int32_t)n && !isnan(vp[k]);
+                            double r = x;  // rollupDelta rollup.go:1859 with a previous value: values[n - 1] - prevValue
+                            if (F == VMB_RF_RATE) {
+                                const uint32_t ex = ((uint32_t)__double2hiint(x) >> 20) & 0x7ffu;
+                                ok = ok && (x == 0.0 || ex - 123u < 1800u);
+                                const double q0 = __dmul_rn(x, rate_R);
+                                const double rem = __fma_rn(-q0, rate_D, x);
+                                r = x == 0.0 ? x : __fma_rn(rem, rate_R, q0);
+                            }
+                            if (ok) {
+                                sc32 += sc_interior;
+                                put(qk, r);
+                            } else {
+                                rest |= 1u << k;
+                            }
+                        }
+                        while (rest) {
+                            const int k = __ffs((int)rest) - 1;
+                            rest &= rest - 1u;
+                            point(q + (uint32_t)k * FU_THREADS);
+                        }
+                    }
+                } else {
+#pragma unroll 2
+                    for (uint32_t q = p + tid; q < p_end; q += FU_THREADS) point(q);
                 }
                 S.s_ser[tid] += scanned + sc32;
             }
             p = p_end;
+            FU_PH(FU_PH_POINTS);
             __syncthreads();
+            FU_PH(FU_PH_WAIT);
             if (p >= P.npoints) continue;
             // ================= slide: keep rows from (first row after tStart(p)) - 1
             {
@@ -1037,7 +1161,12 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                 for (uint32_t q = tid; q < P.npoints; q += FU_THREADS) fu_fold(P.aggr_id, P.aggr_values, P.aggr_counts, cell0 + q, row[q]);
             }
         }
+        FU_PH(FU_PH_SETUP);
     }
+#ifdef VMB_FUSED_PHASES
+    if (lane == 0)
+        for (int k = 0; k < FU_PH_SLOTS; k++) atomicAdd(&fu_phase_cyc[blockIdx.x][k], S.ph[w][k]);
+#endif
     unsigned long long scanned = S.s_thr[tid];
     // block reduce -> one atomic per CTA
     __syncthreads();
@@ -1051,3 +1180,16 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
         if (tot) atomicAdd(P.scanned, tot);
     }
 }
+
+#ifdef VMB_FUSED_PHASES
+// phase-clock build only: copies fu_phase_cyc ([FU_PH_CTAS x FU_PH_SLOTS], cycles summed over the warps of a CTA) to `out`,
+// then zeroes it (reset != 0); returns FU_PH_SLOTS * 1000 + FU_PH_CTAS so that the caller can check the layout
+extern "C" int vmb_fused_phase_cycles(unsigned long long* out, int reset) {
+    if (out && cudaMemcpyFromSymbol(out, fu_phase_cyc, sizeof(fu_phase_cyc)) != cudaSuccess) return -1;
+    if (reset) {
+        static const unsigned long long zero[FU_PH_CTAS][FU_PH_SLOTS] = {};
+        if (cudaMemcpyToSymbol(fu_phase_cyc, zero, sizeof(zero)) != cudaSuccess) return -1;
+    }
+    return FU_PH_SLOTS * 1000 + FU_PH_CTAS;
+}
+#endif
