@@ -553,6 +553,42 @@ int vmb_aggr_rank(vmb_ctx* ctx, int func, int reverse, double* d_vals, size_t ns
                   uint32_t ngroups, const double* ks, double* d_remaining, unsigned char* remaining_nonempty,
                   unsigned char* row_nonempty, uint32_t* out_rows, uint32_t* out_counts, double* scores);
 
+/* count_values("label", q) by (...) (the afe closure of aggr.go:594) on a DEVICE matrix d_vals [nseries x P]; read only, it must
+ * not overlap d_out.  Labels stay with the host, which gets back the exact double that names every output row and formats it
+ * (strconv.FormatFloat(v, 'f', -1, 64)).
+ *   group_ids: HOST, dense ids < ngroups, from the grouping after removing `label` from by (...) or adding it to without (...)
+ *              (:576-592).  Within a group the rows are visited in ascending row order.
+ *   Values:    NaN is skipped; values compare as Go's map[float64] compares them, so -0.0 and +0.0 are ONE key.  The zero row is
+ *              named by the first zero in the reference's loop order (the group's rows in order, then the points): out_value is
+ *              -0.0 exactly when that zero is -0.0.  Every other key has one bit pattern.
+ *   d_out:     [*nout x P]: one row per (group, distinct value), groups ascending, then values ascending (the reference's order is a
+ *              Go map's, so any fixed order is as good; this one is the same on every run).  A cell holds the number of the group's
+ *              rows with that value at that point, NaN where it is 0.  Groups without a value have no rows.
+ *   nout:      in: the capacity of d_out in rows; out: the rows needed.  d_out == NULL or too small: VMB_ERR_CAP, nothing else
+ *              written (a first call with d_out == NULL sizes d_out exactly; the host compares the count with
+ *              -search.maxSeriesPerAggrFunc, :603 / :639, before it allocates anything).
+ *   out_group, out_value: HOST, one per output row: its group; the value that names it.
+ * Bit-identical to the reference.  VMB_ERR_INVALID_ARG for ngroups == 0, a group id >= ngroups, a missing pointer, or nseries /
+ * points > 2^31 - 1, with the outputs untouched; VMB_ERR_NOMEM when the scratch (the sort's as vmb_aggr_order, and 16 bytes per
+ * non-NaN output cell) cannot be had, or for more than 2^32 - 1 non-NaN output cells.  nseries == 0 or points == 0: *nout = 0. */
+int vmb_count_values(vmb_ctx* ctx, const double* d_vals, size_t nseries, size_t points, const uint32_t* group_ids, uint32_t ngroups,
+                     double* d_out, size_t* nout, uint32_t* out_group, double* out_value);
+/* count_values_over_time("label", m[d]) on a series batch: rollupConfig.DoTimeseriesMap (rollup.go:693) with newRollupCountValues
+ * (:1490), the timeseriesMap path of eval.go:957 (subqueries) and :1860 (blocks).  The batch may come from vmb_decode_blocks,
+ * vmb_series_from_host or vmb_series_from_matrix.  The series preamble runs in place as in vmb_rollup, from cfg->flags
+ * (getRollupConfigs sets only VMB_RC_DROP_STALE_NANS for this function); cfg->func_id is not read.  Point p counts the rows
+ * [i_p, j_p) of its window, by the rules of rollupConfig.doInternal (window 0, LookbackDelta, maxPrevInterval) that vmb_rollup uses.
+ *   Keys:      the 'g' string of the value (strconv.FormatFloat(v, 'g', -1, 64)): every NaN is one key ("NaN"), -0.0 and +0.0 are
+ *              two ("-0", "0"), every other key is the exact bits.  A value makes a row only if it lies in some window.
+ *   d_out:     [*nout x P]: one row per (series, key), series ascending, then keys in the order of aggr_order.inc's keys (values
+ *              ascending, -0.0 before +0.0, NaN last).  A cell holds the count of the key in that point's window, NaN where it is 0.
+ *   out_series, out_value: HOST, one per output row: its series; the value that names it (Go's NaN bits for the NaN row).
+ *   nout:      as in vmb_count_values.
+ *   samples_scanned: HOST, may be NULL: what rollupConfig.Do reports, len(values) plus every window's length, summed over series.
+ * Bit-identical to the reference.  Errors as vmb_count_values, plus the vmb_rollup_cfg checks of vmb_rollup (not the func_id). */
+int vmb_rollup_count_values(vmb_ctx* ctx, vmb_series* series, const vmb_rollup_cfg* cfg, double* d_out, size_t* nout,
+                            uint32_t* out_series, double* out_value, uint64_t* samples_scanned);
+
 /* ---- multi-GPU: one process per GPU, the ONE exchange step of the path inside the library (SURVEY 8e) ------------------
  * aggr(rollup(m[d])) by (...): every rank folds its shard of the series into {values, counts}[G x P] (the per-worker
  * incrementalAggrContext, aggr_incremental.go:184), the partial states are merged by one ncclAllReduce per array -- the GPU

@@ -142,6 +142,8 @@ def lib():
                                         u32p]),
         "vmb_buckets_limit": (C.c_int, [vp, vp, sz, sz, u32p, f64p, C.c_uint32, C.c_int64, u32p, C.POINTER(sz)]),
         "vmb_aggr_rank": (C.c_int, [vp, C.c_int, C.c_int, vp, sz, sz, u32p, C.c_uint32, f64p, vp, u8p, u8p, u32p, u32p, f64p]),
+        "vmb_count_values": (C.c_int, [vp, vp, sz, sz, u32p, C.c_uint32, vp, C.POINTER(sz), u32p, f64p]),
+        "vmb_rollup_count_values": (C.c_int, [vp, vp, C.POINTER(RollupCfg), vp, C.POINTER(sz), u32p, f64p, u64p]),
         "vmb_host_alloc": (vp, [sz]),
         "vmb_host_free": (None, [vp]),
         "vmb_ctx_last_stage_ms": (C.c_float, [vp, C.c_int]),

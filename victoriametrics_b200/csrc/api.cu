@@ -85,6 +85,9 @@ struct vmb_ctx {
     DevBuf aggr_state, grp_ids;  // vmb_eval_rollup_aggr_dist: {values, counts}[G x P]; device copy of the per-series group ids
     // vmb_aggr_order / vmb_transform_range: a batch's keys, its merge buffer, per-cell (per-row) statistics, sort plan
     DevBuf oa_keys, oa_keys2, oa_cell, oa_meta;
+    // vmb_count_values / vmb_rollup_count_values: the runs kept across point batches (row ids), per-row / per-group arrays, the
+    // distinct keys
+    DevBuf cv_runs, cv_aux, cv_uniq;
     void* comm = nullptr;     // ncclComm_t (comm.inc); nullptr = single GPU
     bool comm_owned = false;
     int comm_ranks = 1, comm_rank = 0;
@@ -202,7 +205,7 @@ extern "C" void vmb_ctx_destroy(vmb_ctx* c) {
     c->col_cache = nullptr;
     DevBuf* bufs[] = {&c->zscratch, &c->zlit, &c->zstatus, &c->zjobs, &c->zws, &c->args1, &c->args2, &c->rolled,
                       &c->counters, &c->tmp_out, &c->grp, &c->mheap, &c->mnext, &c->zseq, &c->bail, &c->sub_arrays, &c->aggr_state, &c->grp_ids, &c->enc_vals, &c->enc_deltas, &c->enc_out, &c->enc_meta,
-                      &c->oa_keys, &c->oa_keys2, &c->oa_cell, &c->oa_meta};
+                      &c->oa_keys, &c->oa_keys2, &c->oa_cell, &c->oa_meta, &c->cv_runs, &c->cv_aux, &c->cv_uniq};
     for (DevBuf* b : bufs) b->release();
     for (cudaEvent_t e : c->ev)
         if (e) cudaEventDestroy(e);
@@ -1293,19 +1296,16 @@ static int upload_cfg_args(vmb_ctx* ctx, const vmb_rollup_cfg* cfg, int64_t poin
     return 0;
 }
 
-static int run_rollup(vmb_ctx* ctx, vmb_series* s, const vmb_rollup_cfg* cfg, int64_t points, double* d_out,
-                      unsigned long long* d_scanned, const uint32_t* d_out_rows = nullptr, bool record_events = true) {
+// the series preamble (dropStaleNaNs, removeCounterResets, value preFuncs, windows) of cfg on the batch, in place, leaving R set
+// up for a kernel that reads the prepared series
+static int run_preamble(vmb_ctx* ctx, vmb_series* s, const vmb_rollup_cfg* cfg, int64_t points, RollupParams& R) {
     cudaStream_t st = ctx->stream;
-    RollupParams R;
     memset(&R, 0, sizeof(R));
     int rc;
     if ((rc = upload_cfg_args(ctx, cfg, points, &R.cfg))) return rc;
-    R.out_rows = d_out_rows;
     R.meta = s->d_meta;
     R.ts = s->d_ts;
     R.vals = s->d_vals;
-    R.out = d_out;
-    R.scanned = d_scanned;
     R.nseries = (uint32_t)s->nseries;
     R.npoints = (uint32_t)points;
     // data-mutating parts of the preamble run once per batch; a later call must ask for the same mutations (the rows it would
@@ -1343,8 +1343,20 @@ static int run_rollup(vmb_ctx* ctx, vmb_series* s, const vmb_rollup_cfg* cfg, in
     count_launch(ctx);
     if (flags & VMB_RC_DROP_STALE_NANS) s->stale_dropped = true;
     if (flags & VMB_RC_REMOVE_COUNTER_RESETS) s->resets_removed = true;
-    if (ctx->timing && record_events) CU(cudaEventRecord(ctx->ev[ST_ROLLUP], st));
     R.cfg.flags = cfg->flags;
+    return 0;
+}
+
+static int run_rollup(vmb_ctx* ctx, vmb_series* s, const vmb_rollup_cfg* cfg, int64_t points, double* d_out,
+                      unsigned long long* d_scanned, const uint32_t* d_out_rows = nullptr, bool record_events = true) {
+    cudaStream_t st = ctx->stream;
+    RollupParams R;
+    int rc;
+    if ((rc = run_preamble(ctx, s, cfg, points, R))) return rc;
+    R.out_rows = d_out_rows;
+    R.out = d_out;
+    R.scanned = d_scanned;
+    if (ctx->timing && record_events) CU(cudaEventRecord(ctx->ev[ST_ROLLUP], st));
     launch_rollup(R, st);
     count_launch(ctx);
     if (ctx->timing && record_events) CU(cudaEventRecord(ctx->ev[ST_AGGR], st));
@@ -1888,6 +1900,7 @@ extern "C" int vmb_eval_rollup_aggr_device(vmb_ctx* ctx, const vmb_blocks* b, in
 #include "histogram.inc"
 #include "vmrange.inc"
 #include "rank_aggr.inc"
+#include "count_values.inc"
 
 // ------------------------------------------------------------------------------------------------ batched host encoder
 #include <atomic>

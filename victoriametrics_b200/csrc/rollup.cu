@@ -1422,6 +1422,18 @@ __global__ void __launch_bounds__(128) k_series_prepare(RollupParams P) {
     }
 }
 
+// the window of point p, rows [i, j) of a series of n time-sorted rows t (rollup.go:769-777): i = the first row after
+// tEnd - window, j = the first row after tEnd, never below i.  k_rollup's edges of a window it reads from global memory, and
+// the windows of vmb_rollup_count_values.
+struct WinEdges {
+    uint32_t i, j;
+};
+__device__ __forceinline__ WinEdges window_edges(const vmb_rollup_cfg& rc, const SeriesMeta& m, const int64_t* t, uint32_t n, uint32_t p) {
+    const int64_t tEnd = rc.start + (int64_t)p * rc.step;
+    const uint32_t i = upper_bound_ts(t, n, tEnd - m.window), j = upper_bound_ts(t, n, tEnd);
+    return WinEdges{i, j < i ? i : j};
+}
+
 #define ROLLUP_THREADS 256
 #define ROLLUP_CAP 2048    /* rows of one series resident in shared memory */
 #define ROLLUP_SEEKS 2560  /* window edges of one fill: up to ROLLUP_CAP points + window/step shared left edges */
@@ -1699,10 +1711,8 @@ __global__ void __launch_bounds__(ROLLUP_THREADS, 4) k_rollup(RollupParams P) {
                 p_end = min(p + ROLLUP_THREADS, P.npoints);
                 uint32_t q = p + tid;
                 if (q < p_end) {
-                    int64_t tEnd = rc.start + (int64_t)q * rc.step;
-                    uint32_t i = upper_bound_ts(tg, n, tEnd - m.window);
-                    uint32_t j = upper_bound_ts(tg, n, tEnd);
-                    out[q] = rollup_point<F>(rc, m, vg, tg, 0u, n, n, i, j, q, scanned);
+                    const WinEdges w = window_edges(rc, m, tg, n, q);
+                    out[q] = rollup_point<F>(rc, m, vg, tg, 0u, n, n, w.i, w.j, q, scanned);
                 }
                 p = p_end;
                 if (p < P.npoints) {  // restart the resident range at the first row the next point needs

@@ -655,6 +655,97 @@ def go_parse_float(s):
     return None if math.isinf(v) else v
 
 
+def go_format_float(v, fmt):
+    """strconv.FormatFloat(v, fmt, -1, 64) for fmt 'f' and 'g', restated from Go's published documentation: the shortest digits
+    that round-trip (Python's repr digits); 'g' uses %e when the decimal exponent is < -4 or >= 6 (the exponent with at least two
+    digits, as in 1e+06 and 1.5e-05), 'f' never does (772424014, 0.0000001); NaN, +Inf, -Inf and -0."""
+    v = float(v)
+    if math.isnan(v):
+        return "NaN"
+    if math.isinf(v):
+        return "+Inf" if v > 0 else "-Inf"
+    neg = "-" if math.copysign(1.0, v) < 0 else ""
+    if v == 0:
+        return neg + "0"
+    mant, _, ex = repr(abs(v)).partition("e")
+    ip, _, fp = mant.partition(".")
+    digits = ip + fp
+    ds = digits.rstrip("0")
+    e = int(ex or 0) - len(fp) + len(digits) - len(ds)
+    ds = ds.lstrip("0")
+    dp = len(ds) + e  # value = 0.ds x 10^dp
+    if fmt == "g" and not -4 <= dp - 1 < 6:
+        x = dp - 1
+        return "%s%s%s%se%s%02d" % (neg, ds[0], "." if len(ds) > 1 else "", ds[1:], "-" if x < 0 else "+", abs(x))
+    if fmt not in ("f", "g"):
+        raise ValueError("go_format_float: format %r" % fmt)
+    ip = ds[:dp].ljust(dp, "0") if dp > 0 else "0"
+    frac = ("0" * -dp + ds) if dp < 0 else ds[dp:]
+    return neg + ip + ("." + frac if frac else "")
+
+
+def count_values(label, vals_dev_ptr, nseries, points, group_ids, ngroups, device_alloc, ctx=None):
+    """count_values("label", q) by (...) (the afe closure of aggr.go:594, vmb_count_values) on a DEVICE matrix [nseries x points].
+    group_ids: the dense id of every row's label set after removing `label` from by (...) or adding it to without (...).
+    device_alloc(nbytes) -> object with .ptr.  -> (out, n, groups, tags): out holds [n x points] (sized by a first call that only
+    counts, which a caller compares with -search.maxSeriesPerAggrFunc), groups the group of every output row (np.int64), tags the
+    (label, strconv.FormatFloat(v, 'f', -1, 64)) tag every output row adds to its group's labels."""
+    ctx = ctx or _lib.default_context()
+    g = np.ascontiguousarray(group_ids, dtype=np.uint32)
+    if g.size != int(nseries):
+        raise ValueError("count_values: need one group id per series (%d series)" % nseries)
+    nout = C.c_size_t(0)
+    grp, val = np.zeros(1, dtype=np.uint32), np.zeros(1)
+
+    def call(out_ptr):
+        return lib().vmb_count_values(ctx.h, C.c_void_p(int(vals_dev_ptr)), int(nseries), int(points), g.ctypes.data_as(_lib.u32p),
+                                      int(ngroups), out_ptr, C.byref(nout), grp.ctypes.data_as(_lib.u32p), val.ctypes.data_as(_lib.f64p))
+    check(call(None), allow=(-54,))  # VMB_ERR_CAP: the count
+    rows = nout.value
+    grp, val = np.zeros(max(rows, 1), dtype=np.uint32), np.zeros(max(rows, 1))
+    out = device_alloc(max(rows * int(points) * 8, 8))
+    if rows:
+        check(call(C.c_void_p(int(out.ptr))))
+    return out, rows, grp[:rows].astype(np.int64), [(label, go_format_float(v, "f")) for v in val[:rows].tolist()]
+
+
+def count_values_over_time_config(start, end, step, window=0, lookback_delta=0, no_stale_markers=False, min_staleness_interval=0):
+    """the rollupConfig getRollupConfigs (rollup.go:374) makes for count_values_over_time: no window adjustment, no preFunc,
+    dropStaleNaNs unless the series hold no staleness markers.  func_id is not read by vmb_rollup_count_values."""
+    flags = 0 if no_stale_markers else RC_DROP_STALE_NANS
+    if int(step) <= 0 or int(start) > int(end) or int(window) < 0:
+        raise ValueError("BUG: invalid rollupConfig: Step=%d Start=%d End=%d Window=%d" % (step, start, end, window))
+    return RollupCfg(0, flags, int(start), int(end), int(step), int(window), int(lookback_delta), int(min_staleness_interval), 0, 0,
+                     None, None)
+
+
+def count_values_over_time(label, series, start, end, step, window, lookback_delta=0, device_alloc=None, ctx=None,
+                           no_stale_markers=False):
+    """count_values_over_time("label", m[window]) (newRollupCountValues rollup.go:1490 through rollupConfig.DoTimeseriesMap,
+    vmb_rollup_count_values) on a device batch (storage.Series); the series preamble runs in place on it.
+    device_alloc(nbytes) -> object with .ptr.  -> (out, n, series_idx, tags, samples_scanned): out holds [n x points], series_idx
+    the input series of every output row (np.int64), tags the (label, strconv.FormatFloat(v, 'g', -1, 64)) tag it adds to that
+    series' labels."""
+    if device_alloc is None:
+        raise ValueError("count_values_over_time: device_alloc is required")
+    ctx = ctx or series.ctx
+    cfg = count_values_over_time_config(start, end, step, window, lookback_delta, no_stale_markers)
+    points = 1 + (int(end) - int(start)) // int(step)
+    nout = C.c_size_t(0)
+    scanned = C.c_uint64(0)
+    ser, val = np.zeros(1, dtype=np.uint32), np.zeros(1)
+
+    def call(out_ptr):
+        return lib().vmb_rollup_count_values(ctx.h, series.h, C.byref(cfg), out_ptr, C.byref(nout), ser.ctypes.data_as(_lib.u32p),
+                                             val.ctypes.data_as(_lib.f64p), C.byref(scanned))
+    check(call(None), allow=(-54,))
+    rows = nout.value
+    ser, val = np.zeros(max(rows, 1), dtype=np.uint32), np.zeros(max(rows, 1))
+    out = device_alloc(max(rows * points * 8, 8))
+    check(call(C.c_void_p(int(out.ptr))))
+    return out, rows, ser[:rows].astype(np.int64), [(label, go_format_float(v, "g")) for v in val[:rows].tolist()], scanned.value
+
+
 VR_KEEP = 0xFFFFFFFE  # VMB_VR_KEEP
 VR_KINDS = ["kept", "bucket", "gap", "+Inf"]  # enum vmb_vr_kind
 
