@@ -349,8 +349,7 @@ int vmb_binary_op(vmb_ctx* ctx, int op, int is_bool, const double* d_left, const
  * (:516) read from tssRight.  Then, with right_rows[i] = the group of left row i:
  *   `and` (binaryOpAnd :430) / `if` = vmb_binary_op(VMB_BO_IF),  `unless` (:610) / `ifnot` = VMB_BO_IFNOT,  `default` = VMB_BO_DEFAULT;
  * left rows whose key has no right group are dropped (`and`) or kept as they are (`unless`, `default`) by the host's tag matching, which
- * also owns removeEmptySeries (exec.go:193).  `or` (:483) is a union of row sets plus the same fill: left rows, then the right rows of
- * keys the left side lacks. */
+ * also owns removeEmptySeries (exec.go:193).  `or` (:483) fills and clears by metric name instead: vmb_set_or. */
 int vmb_group_first_value(vmb_ctx* ctx, const double* d_vals, size_t nseries, size_t points, const uint32_t* group_ids, uint32_t ngroups,
                           double* d_out);
 
@@ -588,6 +587,45 @@ int vmb_count_values(vmb_ctx* ctx, const double* d_vals, size_t nseries, size_t 
  * Bit-identical to the reference.  Errors as vmb_count_values, plus the vmb_rollup_cfg checks of vmb_rollup (not the func_id). */
 int vmb_rollup_count_values(vmb_ctx* ctx, vmb_series* series, const vmb_rollup_cfg* cfg, double* d_out, size_t* nout,
                             uint32_t* out_series, double* out_value, uint64_t* samples_scanned);
+
+/* removeEmptySeries (exec.go:193) on a DEVICE matrix d_vals [nrows x P], read only: flags (HOST, nrows bytes) = 1 where the row
+ * holds a non-NaN value.  The host builds drop_empty_series (transform.go:1939), limit_offset (:2275) and union (:1725) on it and
+ * on vmb_matrix_merge_rows.  VMB_ERR_INVALID_ARG for a missing pointer or nrows / points > 2^31 - 1, flags untouched.  points == 0:
+ * every flag 0. */
+int vmb_rows_nonempty(vmb_ctx* ctx, const double* d_vals, size_t nrows, size_t points, unsigned char* flags);
+/* sort(q) / sort_desc(q) (newTransformFuncSort transform.go:2557) on a DEVICE matrix d_vals [nrows x P], read only.
+ *   out_rows: HOST, nrows: the rows in output order; vmb_matrix_merge_rows with pb = 0 applies it.
+ *   order    row a comes before row b at the highest point n where they differ, walking n = P - 1 down to 0: a row that is NaN where
+ *            the other is not comes first in both directions; both NaN, or a == b (so -0.0 == +0.0), moves on to n - 1; otherwise
+ *            a < b (desc != 0: b < a) decides.  +-Inf are ordinary values.  Rows equal at every point are equal.
+ * This is a strict weak order, and the library returns its STABLE sort: equal rows keep ascending row order.  That is what Go's
+ * sort.Slice returns for up to 12 rows (its insertion sort) and one of the outcomes of its unstable pdqsort beyond that; rows that
+ * differ at some point are not affected.  VMB_ERR_INVALID_ARG for a missing pointer or nrows / points > 2^31 - 1; VMB_ERR_NOMEM when
+ * the scratch (about 53 bytes per row) cannot be had; out_rows untouched in both cases.  nrows == 0: no-op; points == 0: the
+ * identity. */
+int vmb_sort_rows(vmb_ctx* ctx, const double* d_vals, size_t nrows, size_t points, int desc, uint32_t* out_rows);
+/* `or` (binaryOpOr binary_op.go:483 with fillLeftNaNsWithRightValuesOrMerge :542), in place on two DEVICE matrices d_left [nleft x
+ * P] and d_right [nright x P] (they must not overlap).  Labels stay with the host, which passes ids:
+ *   left_keys, right_keys: HOST, dense ids < nkeys of every row's key (createTimeseriesMapByTagSet :657).
+ *   left_names, right_names: HOST, ids of every row's marshalled sorted metric name: equal ids are names that can be merged.  The
+ *            scalar fast path (:543) applies when a key's right side is one row with an empty name; its rows merge only if the
+ *            key's non-empty left side is one unnamed row.  The host expresses that through the ids: it gives such a right row an id
+ *            no left row has, unless the key's non-empty left side is a single unnamed row.
+ * Per key and point, in the reference's order: the left rows without a non-NaN value (left_nonempty 0, removeEmptySeries :488,
+ * taken before the fill) take no part.  For each other left row in row order, leftIsNaN is read once; then for each right row of
+ * the key in row order, a right row with the same name fills a NaN left value with its current value (the last such row wins, and
+ * a value an earlier left row has cleared is copied as NaN), and the right value becomes NaN if the left value is not NaN or the
+ * names match.  Rows of keys without a non-empty left row, or without a right row, keep their bits.
+ *   left_nonempty, right_nonempty: HOST, nleft / nright bytes: 1 where the row holds a non-NaN value, the left rows before the
+ *            fill, the right rows after it.  The host keeps the left rows with a value, sorted by metric name, then per right key
+ *            all its right rows if no left row has the key (an all-empty left side still has it), otherwise those still
+ *            non-empty, sorted by metric name, and gathers the output with vmb_matrix_merge_rows.
+ * Bit-identical to the reference (a cleared value is Go's NaN).  VMB_ERR_INVALID_ARG for a missing pointer, a key >= nkeys or
+ * nleft / nright / points > 2^31 - 1; VMB_ERR_NOMEM when the scratch cannot be had; the matrices and the flags are untouched in
+ * both cases.  points == 0: every flag 0. */
+int vmb_set_or(vmb_ctx* ctx, double* d_left, size_t nleft, const uint32_t* left_keys, const uint32_t* left_names, double* d_right,
+               size_t nright, const uint32_t* right_keys, const uint32_t* right_names, uint32_t nkeys, size_t points,
+               unsigned char* left_nonempty, unsigned char* right_nonempty);
 
 /* ---- multi-GPU: one process per GPU, the ONE exchange step of the path inside the library (SURVEY 8e) ------------------
  * aggr(rollup(m[d])) by (...): every rank folds its shard of the series into {values, counts}[G x P] (the per-worker

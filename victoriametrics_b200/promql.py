@@ -932,3 +932,145 @@ def aggr_quantile(phis, vals_dev_ptr, nseries, points, out_dev_ptr, group_ids=No
     ph = np.ascontiguousarray(np.broadcast_to(np.asarray(phis, dtype=np.float64), (points,)))
     check(lib().vmb_aggr_quantile(ctx.h, C.c_void_p(int(vals_dev_ptr)), int(nseries), int(points), g.ctypes.data_as(_lib.u32p), int(ngroups),
                                   ph.ctypes.data_as(_lib.f64p), C.c_void_p(int(out_dev_ptr))))
+
+
+def _metric_name_key(labels):
+    """marshalMetricNameSorted (binary_op.go): labels, `__name__` included, as one comparable key"""
+    return tuple(sorted(labels.items()))
+
+
+def _metric_name_order(labels):
+    """metricNameLess exec.go:167: the metric group, then the sorted tags (a prefix first)"""
+    return (labels.get("__name__", ""), tuple(sorted((k, v) for k, v in labels.items() if k != "__name__")))
+
+
+def _gather(src_dev_ptr, rows, points, out_dev_ptr, ctx):
+    """out rows = src rows `rows` (vmb_matrix_merge_rows with pb = 0)"""
+    rows = np.asarray(rows, dtype=np.int64)
+    if rows.size and points:
+        merge_series(src_dev_ptr, rows, points, 0, np.zeros(rows.size, dtype=np.int64), 0, out_dev_ptr, ctx=ctx)
+
+
+def rows_nonempty(vals_dev_ptr, nrows, points, ctx=None):
+    """removeEmptySeries exec.go:193 on a DEVICE matrix [nrows x points] (vmb_rows_nonempty): np.bool_[nrows], True where the
+    row holds a non-NaN value"""
+    ctx = ctx or _lib.default_context()
+    flags = np.zeros(max(int(nrows), 1), dtype=np.uint8)
+    check(lib().vmb_rows_nonempty(ctx.h, C.c_void_p(int(vals_dev_ptr or 0)), int(nrows), int(points), flags.ctypes.data_as(_lib.u8p)))
+    return flags[:int(nrows)].astype(bool)
+
+
+def sort_rows(vals_dev_ptr, nrows, points, desc=False, out_dev_ptr=None, ctx=None):
+    """sort(q) / sort_desc(q) (newTransformFuncSort transform.go:2557, vmb_sort_rows) on a DEVICE matrix [nrows x points]:
+    -> the rows in output order (np.int64), gathered into out_dev_ptr [nrows x points] when it is given"""
+    ctx = ctx or _lib.default_context()
+    order = np.zeros(max(int(nrows), 1), dtype=np.uint32)
+    check(lib().vmb_sort_rows(ctx.h, C.c_void_p(int(vals_dev_ptr or 0)), int(nrows), int(points), int(bool(desc)),
+                              order.ctypes.data_as(_lib.u32p)))
+    order = order[:int(nrows)].astype(np.int64)
+    if out_dev_ptr is not None:
+        _gather(vals_dev_ptr, order, points, out_dev_ptr, ctx)
+    return order
+
+
+def drop_empty_series(vals_dev_ptr, nrows, points, out_dev_ptr=None, ctx=None):
+    """drop_empty_series(q) transform.go:1939: -> the rows that hold a value (np.int64), gathered into out_dev_ptr if given"""
+    rows = np.flatnonzero(rows_nonempty(vals_dev_ptr, nrows, points, ctx=ctx)).astype(np.int64)
+    if out_dev_ptr is not None:
+        _gather(vals_dev_ptr, rows, points, out_dev_ptr, ctx or _lib.default_context())
+    return rows
+
+
+def limit_offset(limit, offset, vals_dev_ptr, nrows, points, out_dev_ptr=None, ctx=None):
+    """limit_offset(limit, offset, q) transform.go:2275: the empty rows removed first, then `offset` rows skipped, then at most
+    `limit` kept -> those rows (np.int64), gathered into out_dev_ptr if given"""
+    if int(limit) < 0 or int(offset) < 0:
+        raise ValueError("limit_offset: limit and offset must not be negative")
+    rows = np.flatnonzero(rows_nonempty(vals_dev_ptr, nrows, points, ctx=ctx)).astype(np.int64)
+    rows = rows[int(offset):int(offset) + int(limit)]
+    if out_dev_ptr is not None:
+        _gather(vals_dev_ptr, rows, points, out_dev_ptr, ctx or _lib.default_context())
+    return rows
+
+
+def union(args, points, out_dev_ptr=None, ctx=None):
+    """union(q1, ...) transform.go:1725.  args: one (dev_ptr, labels of every row) per argument, labels a dict with `__name__`.
+    -> [(arg, row)]: every scalar argument (one unnamed row each) when all of them are scalars, else the first row of every metric
+    name in argument order; gathered into out_dev_ptr [len x points] if given"""
+    ctx = ctx or _lib.default_context()
+    if all(len(lb) == 1 and not lb[0] for _, lb in args):
+        out = [(j, 0) for j in range(len(args))]
+    else:
+        seen, out = set(), []
+        for j, (_, labels) in enumerate(args):
+            for i, lb in enumerate(labels):
+                k = _metric_name_key(lb)
+                if k not in seen:
+                    seen.add(k)
+                    out.append((j, i))
+    if out_dev_ptr is not None:
+        at = 0
+        for j, (ptr, _) in enumerate(args):
+            rows = [i for a, i in out if a == j]
+            _gather(ptr, rows, points, int(out_dev_ptr) + at * int(points) * 8, ctx)
+            at += len(rows)
+    return out
+
+
+def _tagset_key(labels, on, ignoring, keep_metric_names):
+    """the map key of createTimeseriesMapByTagSet binary_op.go:657 (RemoveTagsOn / RemoveTagsIgnoring)"""
+    d = dict(labels)
+    if not keep_metric_names:
+        d.pop("__name__", None)
+    if on is not None:
+        d = {k: v for k, v in d.items() if k in on}
+    elif ignoring:
+        d = {k: v for k, v in d.items() if k not in ignoring}
+    return _metric_name_key(d)
+
+
+def set_or(left_dev_ptr, left_labels, right_dev_ptr, right_labels, points, out_dev_ptr=None, on=None, ignoring=(),
+           keep_metric_names=False, ctx=None):
+    """q1 or q2 (binaryOpOr binary_op.go:483, vmb_set_or) on two DEVICE matrices, filled in place.  left_labels / right_labels: a
+    dict per row, `__name__` included; on / ignoring: the group modifier's labels.  -> [(side, row)] in output order, side 0 for
+    the left matrix and 1 for the right: the left rows with a value sorted by metric name, then the right rows added (all of a key
+    the left side lacks, the ones still holding a value of the others) sorted by metric name.  Gathered into out_dev_ptr
+    [len x points] if given."""
+    ctx = ctx or _lib.default_context()
+    nl, nr = len(left_labels), len(right_labels)
+    keys, names = {}, {}
+    kid = lambda lb: keys.setdefault(_tagset_key(lb, on, ignoring, keep_metric_names), len(keys))
+    nid = lambda lb: names.setdefault(_metric_name_key(lb), len(names))
+    lk = np.array([kid(lb) for lb in left_labels], dtype=np.uint32)
+    rk = np.array([kid(lb) for lb in right_labels], dtype=np.uint32)
+    ln = np.array([nid(lb) for lb in left_labels], dtype=np.uint32)
+    rn = np.array([nid(lb) for lb in right_labels], dtype=np.uint32)
+    # the scalar fast path (:543): a key whose right side is one unnamed row merges only with a single unnamed non-empty left row
+    rcount = np.bincount(rk, minlength=len(keys)) if nr else np.zeros(len(keys), dtype=np.int64)
+    unnamed = nid({})
+    lne_pre = None
+    for r in range(nr):
+        k = rk[r]
+        if rcount[k] != 1 or right_labels[r]:
+            continue
+        left_rows = np.flatnonzero(lk == k)
+        if not (ln[left_rows] == unnamed).any():
+            continue  # no left row has the id: nothing merges either way
+        if lne_pre is None:
+            lne_pre = rows_nonempty(left_dev_ptr, nl, points, ctx=ctx)
+        live = left_rows[lne_pre[left_rows]]
+        if not (live.size == 1 and ln[live[0]] == unnamed):
+            rn[r] = len(names) + r  # an id no left row has
+    lne, rne = np.zeros(max(nl, 1), dtype=np.uint8), np.zeros(max(nr, 1), dtype=np.uint8)
+    u32 = lambda a: np.ascontiguousarray(a, dtype=np.uint32).ctypes.data_as(_lib.u32p)
+    check(lib().vmb_set_or(ctx.h, C.c_void_p(int(left_dev_ptr or 0)), nl, u32(lk), u32(ln), C.c_void_p(int(right_dev_ptr or 0)), nr,
+                           u32(rk), u32(rn), len(keys), int(points), lne.ctypes.data_as(_lib.u8p), rne.ctypes.data_as(_lib.u8p)))
+    left_keys = set(lk.tolist())
+    kept = [i for i in range(nl) if lne[i]]
+    added = [i for i in range(nr) if rk[i] not in left_keys or rne[i]]
+    kept.sort(key=lambda i: (_metric_name_order(left_labels[i]), i))
+    added.sort(key=lambda i: (_metric_name_order(right_labels[i]), i))
+    if out_dev_ptr is not None:
+        _gather(left_dev_ptr, kept, points, out_dev_ptr, ctx)
+        _gather(right_dev_ptr, added, points, int(out_dev_ptr) + len(kept) * int(points) * 8, ctx)
+    return [(0, i) for i in kept] + [(1, i) for i in added]
