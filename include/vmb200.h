@@ -588,6 +588,46 @@ int vmb_count_values(vmb_ctx* ctx, const double* d_vals, size_t nseries, size_t 
 int vmb_rollup_count_values(vmb_ctx* ctx, vmb_series* series, const vmb_rollup_cfg* cfg, double* d_out, size_t* nout,
                             uint32_t* out_series, double* out_value, uint64_t* samples_scanned);
 
+/* VictoriaMetrics' log-scale histogram buckets (metrics.Histogram.Update, vendor/github.com/VictoriaMetrics/metrics/histogram.go:88),
+ * the buckets of histogram(q) and histogram_over_time(m[d]).
+ *   Rule:      NaN and v < 0 are skipped: they count toward no bucket.  Otherwise bucketIdx = (Log10(v) + 9) * 18: < 0 is the
+ *              lower bucket (0, -0.0, +-subnormals, everything below about 1e-9), >= 486 the upper bucket (+Inf included), else
+ *              idx = (unsigned)bucketIdx, one less when bucketIdx is a whole number > 0 (10^n ends its bucket).
+ *   Numbering: 0 the lower bucket "0...1.000e-09"; 1 + idx the decimal bucket idx; 487 the upper bucket "1.000e+18...+Inf".
+ *   Labels:    no strings cross the ABI.  The label of decimal bucket idx is start + "..." + end as initBucketRanges (:220) builds
+ *              them: v = Pow10(-9), start = %.3e of v; for each bucket v *= Pow(10, 1/18), end = %.3e of v, the next start = end.
+ *   Log10:     Go's math.Log10 is Log(x) * (1/Ln10) with Log the fdlibm e_log.c algorithm of math/log.go; the library performs
+ *              those IEEE operations in Go's order with explicit rounding, so its bucket is Go's bit for bit.  One assumption is
+ *              not verified: that Go's amd64 assembly Log (log_amd64.s) gives the bits of the pure-Go code on every input (its
+ *              differing steps are exact, and every subnormal falls in the lower bucket however it is reduced).
+ *
+ * histogram(q) by (...) (aggrFuncHistogram aggr.go:256) on a DEVICE matrix d_vals [nseries x P] (read only; it must not overlap
+ * d_out), up to its final vmrangeBucketsToLE, which is vmb_vmrange_to_le on d_out.
+ *   group_ids: HOST, dense ids < ngroups.
+ *   d_out:     [*nout x P]: one row per (group, bucket hit at some point), groups ascending, then buckets ascending.  A cell holds
+ *              the number of the group's rows in that bucket at that point, and 0 (not NaN) where there is none: the reference
+ *              zero-fills a row when it creates it (:272-275).  A group whose rows hold only NaN or negative values has no rows.
+ *   nout:      in: the capacity of d_out in rows; out: the rows needed.  d_out == NULL or too small: VMB_ERR_CAP, nothing else
+ *              written (a first call with d_out == NULL sizes d_out exactly).
+ *   out_group, out_bucket: HOST, one per output row: its group; its bucket number.
+ * Bit-identical to the reference (counts are whole numbers, so the order of the additions does not matter).
+ * VMB_ERR_INVALID_ARG for ngroups == 0, a group id >= ngroups, a missing pointer, or nseries / points > 2^31 - 1, with the outputs
+ * untouched; VMB_ERR_NOMEM when the scratch (8 bytes per row and 128 per group) cannot be had, or for more than 2^32 - 1 output
+ * rows.  nseries == 0 or points == 0: *nout = 0. */
+int vmb_aggr_histogram(vmb_ctx* ctx, const double* d_vals, size_t nseries, size_t points, const uint32_t* group_ids,
+                       uint32_t ngroups, double* d_out, size_t* nout, uint32_t* out_group, uint32_t* out_bucket);
+/* histogram_over_time(m[d]) on a series batch: rollupConfig.DoTimeseriesMap (rollup.go:693) with rollupHistogram (:1526), the
+ * path of vmb_rollup_count_values with the bucket of a sample as its key: the same batches, the same series preamble from
+ * cfg->flags (getRollupConfigs sets only VMB_RC_DROP_STALE_NANS for this function; cfg->func_id is not read) and the same windows.
+ *   d_out:     [*nout x P]: one row per (series, bucket that occurs in some point's window), series ascending, then buckets
+ *              ascending.  A cell holds the count of the bucket in that point's window, NaN where it is 0 (the rows are copies of
+ *              the origin, whose values are NaN).  A skipped sample (NaN, v < 0) makes no row and counts nowhere.
+ *   out_series, out_bucket: HOST, one per output row: its series; its bucket number.
+ *   nout, samples_scanned: as in vmb_rollup_count_values (skipped samples are scanned).
+ * Bit-identical to the reference, under the assumption stated above.  Errors as vmb_rollup_count_values. */
+int vmb_rollup_histogram(vmb_ctx* ctx, vmb_series* series, const vmb_rollup_cfg* cfg, double* d_out, size_t* nout,
+                         uint32_t* out_series, uint32_t* out_bucket, uint64_t* samples_scanned);
+
 /* removeEmptySeries (exec.go:193) on a DEVICE matrix d_vals [nrows x P], read only: flags (HOST, nrows bytes) = 1 where the row
  * holds a non-NaN value.  The host builds drop_empty_series (transform.go:1939), limit_offset (:2275) and union (:1725) on it and
  * on vmb_matrix_merge_rows.  VMB_ERR_INVALID_ARG for a missing pointer or nrows / points > 2^31 - 1, flags untouched.  points == 0:

@@ -144,6 +144,8 @@ def lib():
         "vmb_aggr_rank": (C.c_int, [vp, C.c_int, C.c_int, vp, sz, sz, u32p, C.c_uint32, f64p, vp, u8p, u8p, u32p, u32p, f64p]),
         "vmb_count_values": (C.c_int, [vp, vp, sz, sz, u32p, C.c_uint32, vp, C.POINTER(sz), u32p, f64p]),
         "vmb_rollup_count_values": (C.c_int, [vp, vp, C.POINTER(RollupCfg), vp, C.POINTER(sz), u32p, f64p, u64p]),
+        "vmb_aggr_histogram": (C.c_int, [vp, vp, sz, sz, u32p, C.c_uint32, vp, C.POINTER(sz), u32p, u32p]),
+        "vmb_rollup_histogram": (C.c_int, [vp, vp, C.POINTER(RollupCfg), vp, C.POINTER(sz), u32p, u32p, u64p]),
         "vmb_rows_nonempty": (C.c_int, [vp, vp, sz, sz, u8p]),
         "vmb_sort_rows": (C.c_int, [vp, vp, sz, sz, C.c_int, u32p]),
         "vmb_set_or": (C.c_int, [vp, vp, sz, u32p, u32p, vp, sz, u32p, u32p, C.c_uint32, sz, u8p, u8p]),

@@ -1901,6 +1901,7 @@ extern "C" int vmb_eval_rollup_aggr_device(vmb_ctx* ctx, const vmb_blocks* b, in
 #include "vmrange.inc"
 #include "rank_aggr.inc"
 #include "count_values.inc"
+#include "vm_histogram.inc"
 #include "rowset.inc"
 
 // ------------------------------------------------------------------------------------------------ batched host encoder

@@ -784,6 +784,11 @@ def prometheus_buckets(vals_dev_ptr, nrows, points, vmranges, has_le, group_ids,
         if fa is None or fb is None:
             continue
         gids[i], starts[i], ends[i], skeys[i], ekeys[i] = int(group_ids[i]), fa, fb, key(a), key(b)
+    return _vmrange_to_le(vals_dev_ptr, n, points, gids, starts, ends, skeys, ekeys, strings, device_alloc, ctx)
+
+
+def _vmrange_to_le(vals_dev_ptr, n, points, gids, starts, ends, skeys, ekeys, strings, device_alloc, ctx):
+    """vmb_vmrange_to_le with the rows' group ids, parsed bounds and string ids -> what prometheus_buckets returns"""
     grouped = gids[gids < VR_KEEP]
     ngroups = int(grouped.max()) + 1 if grouped.size else 0
     nout = C.c_size_t(0)
@@ -804,6 +809,98 @@ def prometheus_buckets(vals_dev_ptr, nrows, points, vmranges, has_le, group_ids,
         check(call(C.c_void_p(int(out.ptr))))
     les = [None if k == 0 else "+Inf" if k == 3 else strings[x] for k, x in zip(kind[:rows].tolist(), le[:rows].tolist())]
     return out, rows, src[:rows].astype(np.int64), kind[:rows].copy(), les
+
+
+VMH_NB = 488  # bucket numbers of vmb_aggr_histogram / vmb_rollup_histogram: 0 lower, 1 + idx decimal, 487 upper
+_VMRANGE_TABLE = None
+
+
+def vmrange_table():
+    """The `vmrange` label of every bucket number, as metrics.Histogram names its buckets (histogram.go:220, initBucketRanges:
+    v = Pow10(-9), then v *= Pow(10, 1/18) once per bucket, every bound formatted %.3e; lowerBucketRange "0...1.000e-09" and
+    upperBucketRange "1.000e+18...+Inf").  Built once.  -> dict with
+      labels[488]                    the label of every bucket number
+      strings                        the distinct bound strings: "0", the 487 decimal bounds (adjacent buckets share one), "+Inf"
+      start_ids, end_ids  uint32[488] every bucket's start / end as an index into strings (the ids vmb_vmrange_to_le takes)
+      starts, ends       float64[488] those strings parsed by strconv.ParseFloat, as vmrangeBucketsToLE parses them"""
+    global _VMRANGE_TABLE
+    if _VMRANGE_TABLE is None:
+        v, mult = 1e-9, 10.0 ** (1.0 / 18)
+        bounds = ["%.3e" % v]
+        for _ in range(VMH_NB - 2):
+            v *= mult
+            bounds.append("%.3e" % v)
+        strings = ["0"] + bounds + ["+Inf"]
+        start_ids = np.arange(VMH_NB, dtype=np.uint32)  # bucket b starts at strings[b] ("0" for the lower bucket)
+        end_ids = start_ids + 1
+        parsed = np.array([go_parse_float(x) for x in strings])
+        _VMRANGE_TABLE = dict(labels=[strings[a] + "..." + strings[a + 1] for a in range(VMH_NB)], strings=strings,
+                              start_ids=start_ids, end_ids=end_ids, starts=parsed[start_ids], ends=parsed[end_ids])
+    return _VMRANGE_TABLE
+
+
+def aggr_histogram_vmrange(vals_dev_ptr, nseries, points, group_ids, ngroups, device_alloc, ctx=None):
+    """histogram(q) by (...) up to its vmrangeBucketsToLE (aggrFuncHistogram aggr.go:256, vmb_aggr_histogram) on a DEVICE matrix
+    [nseries x points].  group_ids: the dense id of every row's label set after the by (...) / without (...) grouping.
+    device_alloc(nbytes) -> object with .ptr.  -> (out, n, groups, buckets): out holds [n x points] counts (0 where none), groups
+    and buckets (np.int64) the group and bucket number of every row; vmrange_table()["labels"] names the buckets."""
+    ctx = ctx or _lib.default_context()
+    g = np.ascontiguousarray(group_ids, dtype=np.uint32)
+    if g.size != int(nseries):
+        raise ValueError("histogram: need one group id per series (%d series)" % nseries)
+    nout = C.c_size_t(0)
+    grp, bkt = np.zeros(1, dtype=np.uint32), np.zeros(1, dtype=np.uint32)
+
+    def call(out_ptr):
+        return lib().vmb_aggr_histogram(ctx.h, C.c_void_p(int(vals_dev_ptr)), int(nseries), int(points), g.ctypes.data_as(_lib.u32p),
+                                        int(ngroups), out_ptr, C.byref(nout), grp.ctypes.data_as(_lib.u32p),
+                                        bkt.ctypes.data_as(_lib.u32p))
+    check(call(None), allow=(-54,))  # VMB_ERR_CAP: the count
+    rows = nout.value
+    grp, bkt = np.zeros(max(rows, 1), dtype=np.uint32), np.zeros(max(rows, 1), dtype=np.uint32)
+    out = device_alloc(max(rows * int(points) * 8, 8))
+    if rows:
+        check(call(C.c_void_p(int(out.ptr))))
+    return out, rows, grp[:rows].astype(np.int64), bkt[:rows].astype(np.int64)
+
+
+def aggr_histogram(vals_dev_ptr, nseries, points, group_ids, ngroups, device_alloc, ctx=None):
+    """histogram(q) by (...) (aggrFuncHistogram aggr.go:256) on a DEVICE matrix [nseries x points]: vmb_aggr_histogram, then its
+    vmrangeBucketsToLE through vmb_vmrange_to_le as prometheus_buckets runs it, the bounds' string ids from vmrange_table().
+    -> (out, n, groups, les): out holds the [n x points] `le` rows, groups the group of every row (np.int64), les its `le`."""
+    ctx = ctx or _lib.default_context()
+    vr, n, groups, buckets = aggr_histogram_vmrange(vals_dev_ptr, nseries, points, group_ids, ngroups, device_alloc, ctx)
+    t = vmrange_table()
+    out, rows, src, _, les = _vmrange_to_le(vr.ptr, n, points, groups.astype(np.uint32), t["starts"][buckets], t["ends"][buckets],
+                                            t["start_ids"][buckets], t["end_ids"][buckets], t["strings"], device_alloc, ctx)
+    return out, rows, groups[src], les
+
+
+def histogram_over_time(series, start, end, step, window, lookback_delta=0, device_alloc=None, ctx=None, no_stale_markers=False):
+    """histogram_over_time(m[window]) (rollupHistogram rollup.go:1526 through rollupConfig.DoTimeseriesMap, vmb_rollup_histogram)
+    on a device batch (storage.Series); the series preamble runs in place on it.  Its rollupConfig is count_values_over_time's.
+    device_alloc(nbytes) -> object with .ptr.  -> (out, n, series_idx, vmranges, samples_scanned): out holds [n x points] (NaN
+    where a bucket has no sample in the window), series_idx the input series of every output row (np.int64), vmranges the
+    `vmrange` label it adds to that series' labels."""
+    if device_alloc is None:
+        raise ValueError("histogram_over_time: device_alloc is required")
+    ctx = ctx or series.ctx
+    cfg = count_values_over_time_config(start, end, step, window, lookback_delta, no_stale_markers)
+    points = 1 + (int(end) - int(start)) // int(step)
+    nout = C.c_size_t(0)
+    scanned = C.c_uint64(0)
+    ser, bkt = np.zeros(1, dtype=np.uint32), np.zeros(1, dtype=np.uint32)
+
+    def call(out_ptr):
+        return lib().vmb_rollup_histogram(ctx.h, series.h, C.byref(cfg), out_ptr, C.byref(nout), ser.ctypes.data_as(_lib.u32p),
+                                          bkt.ctypes.data_as(_lib.u32p), C.byref(scanned))
+    check(call(None), allow=(-54,))
+    rows = nout.value
+    ser, bkt = np.zeros(max(rows, 1), dtype=np.uint32), np.zeros(max(rows, 1), dtype=np.uint32)
+    out = device_alloc(max(rows * points * 8, 8))
+    check(call(C.c_void_p(int(out.ptr))))
+    labels = vmrange_table()["labels"]
+    return out, rows, ser[:rows].astype(np.int64), [labels[b] for b in bkt[:rows].tolist()], scanned.value
 
 
 def buckets_limit(limit, vals_dev_ptr, nrows, points, group_ids, les, ngroups, ctx=None):
