@@ -67,7 +67,7 @@ struct DevBuf {  // grow-only device buffer
 // ev[ST_FUSED] where the aggregate ends, so stage s spans ev[s] .. ev[s + 1]; eval_fused says which events it records.
 enum Stage { ST_ZSTD, ST_DECODE, ST_PREAMBLE, ST_ROLLUP, ST_AGGR, ST_FUSED, ST__COUNT };
 
-#define FUSED_CHUNKS_DEFAULT 4u /* eval_fused: chunks of the fused series list (VMB_FUSED_CHUNKS overrides) */
+#define FUSED_CHUNKS_DEFAULT 2u /* eval_fused: chunks of the fused series list (VMB_FUSED_CHUNKS overrides) */
 #define FUSED_CHUNKS_MAX 64u
 
 struct vmb_ctx {
@@ -97,6 +97,7 @@ struct vmb_ctx {
     uint32_t fused_chunks = 0;  // 0: eval_fused's own choice (fused_chunks()); VMB_FUSED_CHUNKS sets it
     // CTAs per SM of the fused grid (<= FU_CTAS_PER_SM); 0 = FU_CTAS_PER_SM_OVERLAP when chunked, FU_CTAS_PER_SM otherwise
     uint32_t fused_ctas_per_sm = 0;
+    uint32_t huf_ctas_per_sm = 0;  // grid cap of k_huf_decode per SM; 0 = HUF_CTAS_PER_SM (VMB_HUF_CTAS_PER_SM sets it)
     cudaStream_t zstream = nullptr;               // created on first use, non-blocking
     std::vector<cudaEvent_t> zev;                 // zev[k]: the zstd stage of chunk k is done
     int64_t dedup_interval = 0;  // storage.SetDedupInterval (lib/storage/dedup.go:15), ms; 0 = deduplication off
@@ -188,6 +189,10 @@ extern "C" int vmb_ctx_create(int device, vmb_ctx** out) {
     if (const char* s = getenv("VMB_FUSED_CTAS_PER_SM")) {
         const long v = atol(s);
         c->fused_ctas_per_sm = v < 1 ? 1u : (v > FU_CTAS_PER_SM ? (uint32_t)FU_CTAS_PER_SM : (uint32_t)v);
+    }
+    if (const char* s = getenv("VMB_HUF_CTAS_PER_SM")) {
+        const long v = atol(s);
+        c->huf_ctas_per_sm = v < 1 ? 1u : (v > 32 ? 32u : (uint32_t)v);
     }
     for (cudaEvent_t& e : c->ev) CU(cudaEventCreate(&e));
     CU(cudaHostAlloc(&c->h_pinned, 4096, cudaHostAllocDefault));
@@ -718,7 +723,7 @@ static void zstd_huf_range(vmb_ctx* ctx, const vmb_blocks* b, ZstdParams Z, uint
     Z.list = b->d_huf_list + h0;
     Z.count = h1 - h0;
     launch_zstd_prepare(Z, st);
-    launch_huf_decode(Z, st);
+    launch_huf_decode(Z, ctx->huf_ctas_per_sm, st);
     count_launch(ctx, 2);
     if (b->needs_lit) {
         launch_zstd_sequences(Z, st);
@@ -1578,10 +1583,12 @@ static uint32_t fused_chunks(const vmb_ctx* ctx, const vmb_blocks* b) {
 
 static uint32_t fused_ctas_per_sm(const vmb_ctx* ctx, uint32_t C, const vmb_rollup_cfg* cfg) {
     if (ctx->fused_ctas_per_sm) return ctx->fused_ctas_per_sm;
-    // rate()'s fused kernel costs about as much as the zstd stage: giving up a fused CTA per SM to the Huffman kernel pays.  The
-    // heavier functions (avg / max / quantile_over_time: 2-3.5x the zstd stage) lose more on the fused side than the overlap gains
-    // and keep 5; their chunks still overlap where fused CTAs leave room (DESIGN.md section 8)
-    return C > 1 && cfg->func_id == VMB_RF_RATE ? FU_CTAS_PER_SM_OVERLAP : FU_CTAS_PER_SM;
+    // Every function keeps 5: since the Huffman kernel writes its output cooperatively it takes about 3.3 ms of rate()'s 8.4 ms
+    // fused kernel, and giving up a fused CTA per SM to it costs more than the overlap gains (DESIGN.md section 8).  The chunks
+    // still overlap where fused CTAs leave room.
+    (void)C;
+    (void)cfg;
+    return FU_CTAS_PER_SM;
 }
 
 // ctas_per_sm (<= FU_CTAS_PER_SM) caps the grid below what the occupancy calculator allows

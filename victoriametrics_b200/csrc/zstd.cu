@@ -11,7 +11,8 @@
 //   k_huf_decode   : the hot one. Lane-packed: every lane owns ONE Huffman bitstream (4 per frame => 8 frames per
 //                    warp); decode tables (symbol by code prefix, length by symbol) live in shared memory; the
 //                    compressed stream reaches the lane through a private shared-memory ring that is filled by
-//                    warp-uniform 16-byte loads issued two phases ahead; output leaves as aligned 16-byte stores.
+//                    warp-uniform 16-byte loads issued two phases ahead; output is staged in shared memory and written
+//                    out by the whole warp, 4 streams x 128 contiguous bytes per store instruction.
 //   k_zstd_serial  : one thread per frame: (a) executes the sequences section of prepared frames, (b) decodes any
 //                    frame of another shape (raw/RLE blocks, multi-block, raw/RLE/treeless literals) completely.
 #include "common.cuh"
@@ -808,7 +809,55 @@ __global__ void k_zstd_prepare(ZstdParams P) {
 #define HUF_RING 16
 #define HUF_FRAME_BYTES (256 + 64) /* per frame: symbols in canonical order, then 10 thresholds (f32) + 12 index offsets (i16) */
 #define HUF_WARP_TABLE_BYTES (HUF_FRAMES_PER_WARP * HUF_FRAME_BYTES)
+// Output pieces (16 bytes) staged per lane before the warp writes them out together: HUF_STAGE per lane, slot (q, l) of a warp's
+// HUF_STAGE x 32 at q * 32 + (l ^ q * (8 / HUF_STAGE)) -- a step's 32 stores and a write-out's 8-lane groups are conflict-free.
+#ifndef HUF_STAGE
+#define HUF_STAGE 8
+#endif
+#define HUF_STAGE_SLOT(q, l) ((q) * 32 + ((l) ^ ((q) * (8 / HUF_STAGE))))
 #define HUF_FBIAS 0x4B000000u /* bits of 2^23: (HUF_FBIAS | v) is the float 2^23 + v for v < 2^23 */
+#define HUF_CTAS_PER_SM 12u   /* grid cap (VMB_HUF_CTAS_PER_SM overrides it, for measurements) */
+
+// Attribution builds (-DVMB_HUF_EXP=<mask>, scripts/exp_huf_bound.py; never the product): each bit takes one suspect off the
+// symbol loop and keeps the rest of it live.  Their outputs are wrong; they are for timing only.  Without the macro every test
+// below is `if (0)` and the kernel compiles to the product's SASS.
+#ifndef VMB_HUF_EXP
+#define VMB_HUF_EXP 0
+#endif
+#define HUF_EXP_STORE 1     /* no STG.128: the 16-byte pieces are XOR-folded per lane and written once per stream */
+#define HUF_EXP_LOOKUP 2    /* the symbol is cut from the code bits: no perm / adj loads */
+#define HUF_EXP_CONVERT 4   /* the code length from integer compares on packed thresholds: no I2F / F2I */
+#define HUF_EXP_INPUT 8     /* the ring is refilled from registers: no input LDG in the loop */
+#define HUF_EXP_L1 16       /* input loads bypass L1 (ld.global.nc.L1::no_allocate) */
+#define HUF_EXP_PHASES 32   /* clock64() at lane 0 around table build, stream set-up + priming, head, body, tail */
+#define HUF_EXP_CARVEOUT 64 /* shared-memory carveout just large enough for the grid cap: the rest of the SM's 256 KB is L1 */
+#define HUF_EXP(bit) ((VMB_HUF_EXP & (bit)) != 0)
+enum { HUF_PH_BUILD, HUF_PH_PRIME, HUF_PH_HEAD, HUF_PH_BODY, HUF_PH_TAIL, HUF_PH_N, HUF_PH_SYMS = HUF_PH_N, HUF_PH_SLOTS };
+#if HUF_EXP(HUF_EXP_PHASES)
+__device__ unsigned long long huf_phase_cyc[HUF_PH_SLOTS];
+#define HUF_PH(k)                                                                              \
+    do {                                                                                       \
+        const long long ph_c = clock64();                                                      \
+        ph[(k)] += (unsigned long long)(ph_c - ph_t);                                          \
+        ph_t = ph_c;                                                                           \
+    } while (0)
+#else
+#define HUF_PH(k) \
+    do {          \
+    } while (0)
+#endif
+
+// input block load of k_huf_decode (attribution builds may bypass L1)
+__device__ __forceinline__ uint4 huf_ldg(const uint4* p) {
+    if (HUF_EXP(HUF_EXP_L1)) {
+        uint4 r;
+        asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+                     : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
+                     : "l"(p));
+        return r;
+    }
+    return *p;
+}
 
 __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
     // Canonical decode without a 2^log-entry lookup table.  zstd lays a frame's codes out by descending length over the
@@ -824,6 +873,10 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
     uint8_t* wtab = s_smem + (size_t)warp * HUF_WARP_TABLE_BYTES;
     // per-warp input rings behind the tables: HUF_RING words per lane, word-interleaved across lanes
     uint32_t* wring = (uint32_t*)(s_smem + (size_t)HUF_WARPS * HUF_WARP_TABLE_BYTES) + (size_t)warp * HUF_RING * 32;
+#if HUF_EXP(HUF_EXP_PHASES)
+    unsigned long long ph[HUF_PH_SLOTS] = {};
+    long long ph_t = clock64();
+#endif
     for (uint32_t g = blockIdx.x * HUF_WARPS + warp; g < groups; g += gridDim.x * HUF_WARPS) {
         // ---- build the 8 canonical tables cooperatively: symbols in (nbits desc, symbol asc) order
         for (int f = 0; f < HUF_FRAMES_PER_WARP; f++) {
@@ -869,6 +922,7 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
             }
         }
         __syncwarp();
+        HUF_PH(HUF_PH_BUILD);
         // ---- every lane decodes one stream
         {
             const int f = lane >> 2, s = lane & 3;
@@ -877,11 +931,25 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
             const HufJob* job = active ? &P.jobs[ji] : nullptr;
             if (active && (job->nstreams == 0 || s >= job->nstreams)) active = false;
             bool ok = true;
+            // Decoder state, declared here because the body runs as a warp-uniform loop (its stores are cooperative): a lane
+            // that decodes no stream (live == false) runs the loop's votes and stores but none of its decoding.
+            bool live = false;
+            const uint8_t* perm = wtab + f * HUF_FRAME_BYTES;
+            const short* adj = (const short*)(perm + 256 + 40);
+            __half2 th2[5];
+            uint32_t th_i[5] = {0, 0, 0, 0, 0};
+            uint32_t count = 0, total_bits = 0, wr = 0, rd = 0, cand = 0, i = 0;
+            uint8_t* dst = nullptr;
+            const uint4* blk = nullptr;
+            const uint4* blk_min = nullptr;
+            uint32_t* ring = wring + lane;  // slot i -> ring[(i & (HUF_RING - 1)) * 32]
+            uint64_t buf = 0;               // bit buffer, next bit at the top
+            int cnt = 0, cnt_init = 0;      // valid bits in buf; payload bits consumed so far = cnt_init + 32 * rd - cnt
+            uint4 pendA = make_uint4(0, 0, 0, 0), pendB = make_uint4(0, 0, 0, 0);
+            bool hasA = false, hasB = false;
+            uint4 xo = make_uint4(0, 0, 0, 0);  // HUF_EXP_STORE
             if (active) {
-                const uint8_t* perm = wtab + f * HUF_FRAME_BYTES;
-                const short* adj = (const short*)(perm + 256 + 40);
                 // the ten thresholds S_k (0..2048, exact in fp16) as five half2 registers: two compares per instruction
-                __half2 th2[5];
                 {
                     const float* tf = (const float*)(perm + 256);
 #pragma unroll
@@ -890,13 +958,21 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
                         th2[j] = __halves2half2(__ushort2half_rn((unsigned short)a), __ushort2half_rn((unsigned short)b));
                     }
                 }
+                // integer variant: 0x1000 + S_k in each 16-bit half; (th_i[j] - (v + 1) * 0x10001) has bit 12 (28) set iff v < S_k
+                if (HUF_EXP(HUF_EXP_CONVERT)) {
+                    const float* tf = (const float*)(perm + 256);
+#pragma unroll
+                    for (int j = 0; j < 5; j++)
+                        th_i[j] = ((0x1000u + (__float_as_uint(tf[2 * j + 1]) & 0x7fffffu)) << 16) |
+                                  (0x1000u + (__float_as_uint(tf[2 * j]) & 0x7fffffu));
+                }
                 uint32_t regen = job->regen_size;
                 uint32_t seg = job->nstreams == 1 ? regen : (regen + 3) / 4;
-                uint32_t count = job->nstreams == 1 ? regen : (s < 3 ? seg : regen - 3 * seg);
+                count = job->nstreams == 1 ? regen : (s < 3 ? seg : regen - 3 * seg);
                 uint64_t soff = job->src_off;
                 for (int k = 0; k < s; k++) soff += job->stream_size[k];
                 uint32_t slen = job->stream_size[s];
-                uint8_t* dst = (job->dst_is_lit ? P.lit : P.scratch) + job->dst_off + (size_t)s * seg;
+                dst = (job->dst_is_lit ? P.lit : P.scratch) + job->dst_off + (size_t)s * seg;
                 const uint8_t* base = P.payload + soff;
                 uint32_t last = slen ? base[slen - 1] : 0;
                 if (count == 0) {
@@ -904,6 +980,7 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
                 } else if (slen == 0 || last == 0) {
                     ok = false;
                 } else {
+                    live = true;
                     // Backward bitstream, lane-private, with every memory access at a warp-uniform program point:
                     //   * the stream is pulled in as aligned 16-byte blocks (LDG.128) that land in registers and are moved
                     //     into the lane's shared-memory ring TWO phases (16 symbols) later -- the HBM round trip is covered
@@ -911,14 +988,10 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
                     //   * 32-bit words are popped from the ring into an MSB-aligned 64-bit bit buffer; the candidate word is
                     //     re-read (LDS) at every refill check by all lanes, so that read is uniform too.
                     // The ring is word-interleaved across lanes (word w of lane l at [w*32 + l]): conflict-free.
-                    const uint32_t total_bits = (slen - 1) * 8 + (uint32_t)hb32(last);
+                    total_bits = (slen - 1) * 8 + (uint32_t)hb32(last);
                     const uint8_t* endp = base + slen - 1;                                 // byte holding the final-bit marker
-                    const uint4* blk = (const uint4*)((uintptr_t)endp & ~(uintptr_t)15);   // aligned block that holds it
-                    const uint4* blk_min = (const uint4*)(((uintptr_t)base & ~(uintptr_t)15) - 32);  // never read below this
-                    uint32_t* ring = wring + lane;  // slot i -> ring[(i & (HUF_RING - 1)) * 32]
-                    uint32_t wr = 0, rd = 0;        // words written / consumed
-                    uint64_t buf;                   // bit buffer, next bit at the top
-                    int cnt;                        // valid bits in buf
+                    blk = (const uint4*)((uintptr_t)endp & ~(uintptr_t)15);   // aligned block that holds it
+                    blk_min = (const uint4*)(((uintptr_t)base & ~(uintptr_t)15) - 32);  // never read below this
                     {
                         uint4 q = *blk;
                         uint64_t qlo = ((uint64_t)q.y << 32) | q.x, qhi = ((uint64_t)q.w << 32) | q.z;
@@ -946,7 +1019,7 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
 #pragma unroll
                         for (int k = 0; k < 3; k++) {
                             if (blk > blk_min) blk--;
-                            uint4 b = *blk;
+                            uint4 b = huf_ldg(blk);
                             ring[((wr + 0) & (HUF_RING - 1)) * 32] = b.w;
                             ring[((wr + 1) & (HUF_RING - 1)) * 32] = b.z;
                             ring[((wr + 2) & (HUF_RING - 1)) * 32] = b.y;
@@ -954,10 +1027,8 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
                             wr += 4;
                         }
                     }
-                    const int cnt_init = cnt;  // payload bits consumed so far = cnt_init + 32 * rd - cnt (no per-symbol counter)
-                    uint4 pendA = make_uint4(0, 0, 0, 0), pendB = make_uint4(0, 0, 0, 0);
-                    bool hasA = false, hasB = false;
-                    uint32_t cand = ring[(rd & (HUF_RING - 1)) * 32];
+                    cnt_init = cnt;
+                    cand = ring[(rd & (HUF_RING - 1)) * 32];
 #define HUF_PHASE(pend, has)                                                               \
     do {                                                                                   \
         if (has) { /* block fetched two phases ago: now in registers for sure */           \
@@ -971,7 +1042,8 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
         has = (wr - rd) + 8u <= (uint32_t)HUF_RING;                                        \
         if (has) {                                                                         \
             if (blk > blk_min) blk--;                                                      \
-            pend = *blk;                                                                   \
+            if (HUF_EXP(HUF_EXP_INPUT)) pend = make_uint4(rd, wr, (uint32_t)cnt, (uint32_t)(uintptr_t)blk); \
+            else pend = huf_ldg(blk);                                                      \
         }                                                                                  \
         cand = ring[(rd & (HUF_RING - 1)) * 32]; /* the slot may have been written just now */ \
     } while (0)
@@ -985,19 +1057,28 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
         cand = ring[(rd & (HUF_RING - 1)) * 32];                                           \
     } while (0)
 #define HUF_LT(k) __hlt2(vv_, th2[k]) /* (1.0, 0.0) per half */
+#define HUF_LTI(j) ((th_i[j] - v1_) & 0x10001000u)
 #define HUF_SYM(outv, shift)                                                               \
     do {                                                                                   \
         const uint32_t v_ = (uint32_t)(buf >> 53);                                         \
-        const __half2 vv_ = __half2half2(__ushort2half_rn((unsigned short)v_));            \
-        /* code length = 1 + #{k : v < S_k}; the count (<= 10) is exact in fp16 */          \
-        const __half2 c_ = __hadd2(__hadd2(__hadd2(HUF_LT(0), HUF_LT(1)), __hadd2(HUF_LT(2), HUF_LT(3))), HUF_LT(4)); \
-        const uint32_t nb_ = 1u + (uint32_t)__half2ushort_rz(__hadd(__low2half(c_), __high2half(c_))); \
+        uint32_t nb_;                                                                      \
+        if (HUF_EXP(HUF_EXP_CONVERT)) {                                                    \
+            const uint32_t v1_ = (v_ + 1u) * 0x10001u;                                     \
+            const uint32_t a_ = HUF_LTI(0) + HUF_LTI(1) + HUF_LTI(2) + HUF_LTI(3) + HUF_LTI(4); \
+            nb_ = 1u + ((a_ * 0x10001u) >> 28);                                            \
+        } else {                                                                           \
+            const __half2 vv_ = __half2half2(__ushort2half_rn((unsigned short)v_));        \
+            /* code length = 1 + #{k : v < S_k}; the count (<= 10) is exact in fp16 */      \
+            const __half2 c_ = __hadd2(__hadd2(__hadd2(HUF_LT(0), HUF_LT(1)), __hadd2(HUF_LT(2), HUF_LT(3))), HUF_LT(4)); \
+            nb_ = 1u + (uint32_t)__half2ushort_rz(__hadd(__low2half(c_), __high2half(c_))); \
+        }                                                                                  \
         buf <<= nb_;                                                                       \
         cnt -= (int)nb_;                                                                   \
-        const uint32_t sym_ = perm[((v_ >> (HUF_MAX_LOG - nb_)) + (uint32_t)(int)adj[nb_]) & 255u]; \
+        const uint32_t sym_ = HUF_EXP(HUF_EXP_LOOKUP) ? ((v_ >> (HUF_MAX_LOG - nb_)) & 255u)  \
+            : perm[((v_ >> (HUF_MAX_LOG - nb_)) + (uint32_t)(int)adj[nb_]) & 255u];         \
         outv |= sym_ << (shift);                                                           \
     } while (0)
-                    uint32_t i = 0;
+                    HUF_PH(HUF_PH_PRIME);
                     // head: single bytes until dst is 16-byte aligned (<= 15 symbols <= 6 words: covered by the primed ring)
                     while (i < count && (((uintptr_t)(dst + i)) & 15)) {
                         HUF_REFILL();
@@ -1005,8 +1086,19 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
                         HUF_SYM(o, 0);
                         dst[i++] = (uint8_t)o;
                     }
-                    // body: 16 symbols per aligned 128-bit store = two phases of 8 symbols (<= 88 bits <= 3 words each)
-                    for (; i + 16 <= count; i += 16) {
+                    HUF_PH(HUF_PH_HEAD);
+                }
+            }
+            // body: 16 symbols per aligned 16-byte piece = two phases of 8 symbols (<= 88 bits <= 3 words each).  A lane's
+            // pieces are staged in shared memory; every HUF_STAGE steps the warp writes them out, each store instruction
+            // covering 32 / HUF_STAGE streams with HUF_STAGE consecutive pieces each, instead of 32 streams with one piece.
+            {
+                uint4* stage = (uint4*)(s_smem + (size_t)HUF_WARPS * (HUF_WARP_TABLE_BYTES + HUF_RING * 32 * sizeof(uint32_t))) +
+                               warp * HUF_STAGE * 32;
+                uint32_t k = 0, bi = i;  // steps of this batch; the lane's output index at the batch's start
+                for (;;) {
+                    const bool more = live && i + 16 <= count;
+                    if (more) {
                         uint32_t o[4];
                         HUF_PHASE(pendA, hasA);
 #pragma unroll
@@ -1030,8 +1122,36 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
                             HUF_SYM(o[q], 16);
                             HUF_SYM(o[q], 24);
                         }
-                        *(uint4*)(dst + i) = make_uint4(o[0], o[1], o[2], o[3]);
+                        if (HUF_EXP(HUF_EXP_STORE)) {
+                            xo.x ^= o[0]; xo.y ^= o[1]; xo.z ^= o[2]; xo.w ^= o[3];
+                        } else {
+                            stage[HUF_STAGE_SLOT(k, lane)] = make_uint4(o[0], o[1], o[2], o[3]);
+                        }
+                        i += 16;
                     }
+                    const bool any = __any_sync(VMB_FULL, more);
+                    if (++k == HUF_STAGE || !any) {  // write the batch: piece q of stream l goes to dst_l + bi_l + 16 q
+                        __syncwarp();
+                        const uint32_t n_l = (i - bi) >> 4;
+                        const uintptr_t p_l = (uintptr_t)(dst + bi);
+#pragma unroll
+                        for (int j = 0; j < HUF_STAGE; j++) {
+                            const int l = (j * 32 + lane) / HUF_STAGE, q = (j * 32 + lane) % HUF_STAGE;
+                            const uint32_t n = __shfl_sync(VMB_FULL, n_l, l);
+                            const uintptr_t pp = (uintptr_t)__shfl_sync(VMB_FULL, (unsigned long long)p_l, l);
+                            if ((uint32_t)q < n && !HUF_EXP(HUF_EXP_STORE)) *(uint4*)(pp + 16 * q) = stage[HUF_STAGE_SLOT(q, l)];
+                        }
+                        __syncwarp();
+                        k = 0;
+                        bi = i;
+                    }
+                    if (!any) break;
+                }
+            }
+            if (HUF_EXP(HUF_EXP_STORE) && live && i >= 16) *(uint4*)(dst + i - 16) = xo;
+            if (live) {
+                {
+                    HUF_PH(HUF_PH_BODY);
                     // tail (<= 15 symbols <= 6 words): what is already in the ring plus the pending blocks is enough
                     if (i < count) {
                         HUF_PHASE(pendA, hasA);
@@ -1044,19 +1164,31 @@ __global__ void __launch_bounds__(HUF_WARPS * 32) k_huf_decode(ZstdParams P) {
                         HUF_SYM(o, 0);
                         dst[i] = (uint8_t)o;
                     }
+                    HUF_PH(HUF_PH_TAIL);
+#if HUF_EXP(HUF_EXP_PHASES)
+                    ph[HUF_PH_SYMS] += count;
+#endif
 #undef HUF_PHASE
 #undef HUF_REFILL
 #undef HUF_SYM
 #undef HUF_LT
+#undef HUF_LTI
                     ok = (long long)cnt_init + 32ll * (long long)rd - (long long)cnt == (long long)total_bits;
                 }
             }
             // a frame fails if any of its streams failed
+            // variants that write wrong literals fail every frame, so that no later kernel reads them
+            if (HUF_EXP(HUF_EXP_STORE | HUF_EXP_LOOKUP | HUF_EXP_INPUT)) ok = false;
             uint32_t bad = __ballot_sync(VMB_FULL, active && !ok);
+            if (HUF_EXP(HUF_EXP_STORE | HUF_EXP_LOOKUP | HUF_EXP_INPUT) && ji < P.count && s == 0) bad |= 1u << (f * 4);
             if (ji < P.count && s == 0 && ((bad >> (f * 4)) & 0xf)) P.status[P.jobs[ji].col] = VMB_ERR_ZSTD;
         }
         __syncwarp();
     }
+#if HUF_EXP(HUF_EXP_PHASES)
+    if (lane == 0)  // lane 0's cycles; the wait for the warp's slower lanes lands in the next table build
+        for (int k = 0; k < HUF_PH_SLOTS; k++) atomicAdd(&huf_phase_cyc[k], ph[k]);
+#endif
 }
 
 // ---- sequences of prepared frames, in two kernels.
@@ -1585,18 +1717,38 @@ void launch_zstd_prepare(const ZstdParams& P, cudaStream_t st) {
     k_zstd_prepare<<<(P.count + 63) / 64, 64, 0, st>>>(P);
 }
 
-void launch_huf_decode(const ZstdParams& P, cudaStream_t st) {
+// ctas_per_sm: grid cap per SM, 0 = HUF_CTAS_PER_SM
+void launch_huf_decode(const ZstdParams& P, uint32_t ctas_per_sm, cudaStream_t st) {
     if (!P.count) return;
-    // 9 KB per CTA: below the 48 KB that need no opt-in.  The grid is capped at 12 CTAs (24 warps) per SM, not the 16 that
-    // registers and shared memory would allow: fewer resident decoders measured faster (the flagship's one-shot zstd stage
-    // 5.92 ms against 6.38 ms with 16, on an H100 SXM at 700 W), and beside the fused kernel only 4 fit anyway.
-    constexpr size_t smem = (size_t)HUF_WARPS * HUF_WARP_TABLE_BYTES + (size_t)HUF_WARPS * HUF_RING * 32 * sizeof(uint32_t);
+    // 17 KB per CTA (tables, input rings, output staging): below the 48 KB that need no opt-in.  The grid is capped at 12 CTAs
+    // (24 warps) per SM: with the cooperative stores the flagship's one-shot k_huf_decode measured 3.31 ms at 12, 3.23 at 4 and
+    // 3.40 at 16 (H100 SXM, 700 W; DESIGN.md section 8).
+    constexpr size_t smem = (size_t)HUF_WARPS * HUF_WARP_TABLE_BYTES + (size_t)HUF_WARPS * HUF_RING * 32 * sizeof(uint32_t) +
+                            (size_t)HUF_WARPS * HUF_STAGE * 32 * sizeof(uint4);
     static_assert(smem <= 48 * 1024, "k_huf_decode would need cudaFuncAttributeMaxDynamicSharedMemorySize");
+    const uint32_t cap = ctas_per_sm ? ctas_per_sm : HUF_CTAS_PER_SM;
+    if (HUF_EXP(HUF_EXP_CARVEOUT)) {  // percent of the 228 KB maximum; each CTA also takes 1 KB the system reserves
+        const int pct = (int)((cap * (smem + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024));
+        cudaFuncSetAttribute(k_huf_decode, cudaFuncAttributePreferredSharedMemoryCarveout, pct > 100 ? 100 : pct);
+    }
     uint32_t groups = (P.count + HUF_FRAMES_PER_WARP - 1) / HUF_FRAMES_PER_WARP;
     uint32_t grid = (groups + HUF_WARPS - 1) / HUF_WARPS;
-    if (grid > VMB_SMS * 12u) grid = VMB_SMS * 12u;
+    if (grid > VMB_SMS * cap) grid = VMB_SMS * cap;
     k_huf_decode<<<grid, HUF_WARPS * 32, smem, st>>>(P);
 }
+
+#if HUF_EXP(HUF_EXP_PHASES)
+// phase-clock build only: copies huf_phase_cyc (lane 0's cycles summed over all warps, then lane 0's symbols) to `out`, then
+// zeroes it (reset != 0); returns HUF_PH_SLOTS so that the caller can check the layout
+extern "C" int vmb_huf_phase_cycles(unsigned long long* out, int reset) {
+    if (out && cudaMemcpyFromSymbol(out, huf_phase_cyc, sizeof(huf_phase_cyc)) != cudaSuccess) return -1;
+    if (reset) {
+        static const unsigned long long zero[HUF_PH_SLOTS] = {};
+        if (cudaMemcpyToSymbol(huf_phase_cyc, zero, sizeof(zero)) != cudaSuccess) return -1;
+    }
+    return HUF_PH_SLOTS;
+}
+#endif
 
 void launch_zstd_sequences(const ZstdParams& P, cudaStream_t st) {
     if (!P.count || !P.ws_count || !P.seq_rec) return;
