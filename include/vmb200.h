@@ -359,12 +359,27 @@ int vmb_group_first_value(vmb_ctx* ctx, const double* d_vals, size_t nseries, si
  * addition order is part of the result).  arg1 / arg2: HOST arrays of `points` values = getScalar of the scalar arguments:
  *   clamp(q, min, max): arg1 = min, arg2 = max;  clamp_min / clamp_max: arg1;  round(q, nearest): arg1 = nearest, arg2 =
  *   math.Pow10(-e) with (_, e) = decimal.FromFloat(nearest) (transform.go:2341; vmb_float_to_decimal gives e).
- *   smooth_exponential(q, sf): arg1 = sf (getScalar(args[1], 1)).  Others: NULL.
+ *   smooth_exponential(q, sf): arg1 = sf (getScalar(args[1], 1)).  bitmap_and / or / xor(q, w): arg1 = w.  Others: NULL.
  * smooth_exponential (:1664): leading NaNs, then leading +-Infs are skipped (if nothing but +-Infs follows, nothing is cut); avg
  * starts at the first kept value, which stays as it is; later NaNs stay, a later +-Inf becomes the current avg, any other v
  * becomes avg = avg*(1-sf) + v*sf with sf = arg1 at the point's own index, NaN -> 1, clamped to [0, 1].
+ * Date-time functions hour, minute, day_of_month, day_of_week, day_of_year, days_in_month, month, year (newTransformFuncDateTime
+ * :333): a NaN stays as it is (:347); any other v becomes the field of time.Unix(int64(v), 0).UTC() as a double: hour = sod / 3600,
+ * minute = sod / 60 % 60 with sod the second of the UTC day (floor semantics before 1970), day_of_week 0 = Sunday, day_of_year
+ * 1..366, year astronomical (year 0 exists; negative years), days_in_month the reference's table with its leap test on
+ * uint32(year) (:2874: February of year -100 has 29 days).  The zero-argument forms are these on time()'s one-row matrix.
+ * Bitmap functions bitmap_and / or / xor(q, w) (newTransformBitmap :2724): NaN (math.NaN()) where v or w is NaN, else
+ * float64(op(uint64(v), uint64(w))), rounded to nearest even.
+ * Two Go-platform assumptions fix what Go leaves to the implementation, both unverified for want of a Go toolchain:
+ *   - conversions as on amd64 at the default GOAMD64 level: int64(v) = trunc(v) for -2^63 <= v < 2^63, else -2^63 (+-Inf
+ *     included; CVTTSD2SQ); uint64(v) = uint64(int64(v)) for v < 2^63 (-1.5 -> 2^64 - 1, -Inf -> 2^63), else
+ *     uint64(int64(v - 2^63)) | 2^63 ([2^63, 2^64) exact, >= 2^64 and +Inf -> 2^63) -- ssagen's float64ToUint64;
+ *   - Go 1.26's time arithmetic (the reference's go.mod): abs = uint64(s + 9223372028741760000) seconds since March 1 of year
+ *     -292277022400 (absoluteYears), split in uint64.  For s >= -9223372028741760000 that is the proleptic Gregorian calendar
+ *     (the verified domain: every int64 second but the lowest 8.1e9); below it, -2^63 included, the sum wraps and the fields
+ *     follow Go's wrapped arithmetic (csrc/go_conv.cuh restates it).
  * exp / ln / log2 / log10 / trigonometric / hyperbolic functions are the CUDA math library's (<= 2 ulp from Go's); everything else is
- * bit-exact. */
+ * bit-exact.  VMB_ERR_INVALID_ARG for ids 27..31, 47..63, >= 75 and for a missing argument array. */
 enum vmb_transform_func {
     VMB_TF_ABS = 0, VMB_TF_CEIL, VMB_TF_FLOOR, VMB_TF_SQRT, VMB_TF_EXP, VMB_TF_LN, VMB_TF_LOG2, VMB_TF_LOG10, VMB_TF_SIN, VMB_TF_COS,
     VMB_TF_TAN, VMB_TF_ASIN, VMB_TF_ACOS, VMB_TF_ATAN, VMB_TF_SINH, VMB_TF_COSH, VMB_TF_TANH, VMB_TF_ASINH, VMB_TF_ACOSH, VMB_TF_ATANH,
@@ -373,7 +388,10 @@ enum vmb_transform_func {
      * keep_last_value / keep_next_value (:1214, :1237), remove_resets = removeCounterResetsMaybeNaNs (:2906) */
     VMB_TF_RUNNING_SUM = 32, VMB_TF_RUNNING_MIN, VMB_TF_RUNNING_MAX, VMB_TF_RUNNING_AVG, VMB_TF_RANGE_SUM, VMB_TF_RANGE_MIN,
     VMB_TF_RANGE_MAX, VMB_TF_RANGE_AVG, VMB_TF_RANGE_FIRST, VMB_TF_RANGE_LAST, VMB_TF_KEEP_LAST_VALUE, VMB_TF_KEEP_NEXT_VALUE,
-    VMB_TF_REMOVE_RESETS, VMB_TF_INTERPOLATE /* :1261 */, VMB_TF_SMOOTH_EXPONENTIAL /* :1664 */
+    VMB_TF_REMOVE_RESETS, VMB_TF_INTERPOLATE /* :1261 */, VMB_TF_SMOOTH_EXPONENTIAL /* :1664 */,
+    /* date-time (:1171 hour, :2314 minute, :2318 month, :2785 year, :360-376 the rest) and bitmap (:2710-2744) functions */
+    VMB_TF_HOUR = 64, VMB_TF_MINUTE, VMB_TF_DAY_OF_MONTH, VMB_TF_DAY_OF_WEEK, VMB_TF_DAY_OF_YEAR, VMB_TF_DAYS_IN_MONTH, VMB_TF_MONTH,
+    VMB_TF_YEAR, VMB_TF_BITMAP_AND, VMB_TF_BITMAP_OR, VMB_TF_BITMAP_XOR
 };
 int vmb_transform(vmb_ctx* ctx, int func, double* d_matrix, size_t nrows, size_t points, const double* arg1, const double* arg2);
 /* The transforms that reduce a whole series and then rewrite it (app/vmselect/promql/transform.go), in place on a DEVICE matrix

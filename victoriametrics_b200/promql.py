@@ -506,6 +506,9 @@ TRANSFORM_FUNCS = {n: i for i, n in enumerate(
 TRANSFORM_FUNCS.update({n: 32 + i for i, n in enumerate(
     ["running_sum", "running_min", "running_max", "running_avg", "range_sum", "range_min", "range_max", "range_avg", "range_first",
      "range_last", "keep_last_value", "keep_next_value", "remove_resets", "interpolate", "smooth_exponential"])})
+TRANSFORM_FUNCS.update({n: 64 + i for i, n in enumerate(
+    ["hour", "minute", "day_of_month", "day_of_week", "day_of_year", "days_in_month", "month", "year", "bitmap_and", "bitmap_or",
+     "bitmap_xor"])})
 
 
 def _go_pow10(n):
@@ -520,14 +523,15 @@ def _go_pow10(n):
 def transform(name, dev_ptr, nrows, points, *scalar_args, ctx=None):
     """transform.go value functions in place on a DEVICE matrix [nrows x points] (vmb_transform).  scalar_args: the function's scalar
     arguments (numbers or per-point arrays, getScalar): clamp(min, max), clamp_min(min), clamp_max(max), round(nearest = 1),
-    smooth_exponential(sf)"""
+    smooth_exponential(sf), bitmap_and / bitmap_or / bitmap_xor(w).  The zero-argument date-time forms (`hour()` = `hour(time())`)
+    are this call on a one-row matrix of float64(ts) / 1e3 over the query's timestamps (evalTime, eval.go:1959)."""
     ctx = ctx or _lib.default_context()
     name = name.lower()
     bc = lambda x: np.ascontiguousarray(np.broadcast_to(np.asarray(x, dtype=np.float64), (points,)))
     a1 = a2 = None
     if name == "clamp":
         a1, a2 = bc(scalar_args[0]), bc(scalar_args[1])
-    elif name in ("clamp_min", "clamp_max", "smooth_exponential"):
+    elif name in ("clamp_min", "clamp_max", "smooth_exponential", "bitmap_and", "bitmap_or", "bitmap_xor"):
         a1 = bc(scalar_args[0])
     elif name == "round":
         a1 = bc(scalar_args[0] if scalar_args else 1.0)
