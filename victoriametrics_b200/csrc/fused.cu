@@ -80,6 +80,21 @@ __device__ unsigned long long fu_phase_cyc[FU_PH_CTAS][FU_PH_SLOTS];
 #define FU_PH_COUNT(k) ((void)0)
 #endif
 
+// Attribution builds (-DVMB_FUSED_EXP=<mask>, scripts/exp_fused_bound.py; never the product): each bit takes one suspect off
+// the per-row loops while the rest stays live.  Their outputs may be wrong; their bails are the product's.  Without the macro
+// the kernel compiles to the same SASS.
+//    1 store     no per-point store: the points are XOR-folded into a register, one store per thread and series
+//    2 conflict  the raw deltas of a tile without long varints go to a lane-major int32 array (conflict-free) instead of the
+//                ring, and the emit reads them there: 16 KB more per CTA, so fewer CTAs fit
+//    4 order     the emit's and the interior points' loads of the next step are issued before the current step's stores
+//                (software-pipelined; the loads are not volatile and the emit's stores have no memory clobber)
+//    8 guards    the emit's full four-row batches run without the per-row guards, reset candidates and special-value test
+//   16 rcr       no counter-reset pass over the rows (one-pass correction, event path); the emit still finds the candidates
+#ifndef VMB_FUSED_EXP
+#define VMB_FUSED_EXP 0
+#endif
+#define FU_EXP(b) ((VMB_FUSED_EXP & (b)) != 0)
+
 struct FusedParams {
     const vmb_block_desc* descs;
     const ColInfo* cols;
@@ -131,6 +146,7 @@ struct FusedSmem {
     double ev_amt[FU_MAX_EVENTS], ev_cum[FU_MAX_EVENTS];
     uint32_t ev_row[FU_MAX_EVENTS];
     uint32_t nev;
+    uint32_t rcr_mode;  // how the fill's corrections are applied (thread 0 decides, behind the barrier everybody reads it)
     unsigned long long nd_v, nd_d1;  // nearest-delta(2) state in front of the next fill: last value, last delta
     uint32_t flags;  // bit 0: bail (set while parsing, read behind the barrier that ends the parse)
     uint32_t flags_emit;  // the same for the emit pass: a word of its own, so that a warp already emitting cannot race a warp still reading `flags`
@@ -140,6 +156,9 @@ struct FusedSmem {
     FuSeries ser;  // the current series (read where it is used: it stays valid for the whole series)
 #ifdef VMB_FUSED_PHASES
     unsigned long long ph[FU_WARPS][FU_PH_SLOTS];
+#endif
+#if FU_EXP(2)
+    int32_t raw32[32][FU_THREADS];  // [k][thread]: the lane's k-th raw delta of the fill (a lane has <= 32 rows per fill)
 #endif
 };
 
@@ -219,6 +238,35 @@ __device__ __forceinline__ long long fu_lds_i64(uint32_t val_s, uint32_t row) {
 __device__ __forceinline__ void fu_sts_i64(uint32_t val_s, uint32_t row, long long v) {
     asm volatile("st.shared.b64 [%0], %1;" ::"r"(val_s + fu_swz_b(row)), "l"(v) : "memory");
 }
+// the aligned 16-byte slot pair of rows 2m and 2m + 1 (row = 2m; which of the two is .x depends on the swizzle)
+__device__ __forceinline__ double2 fu_lds2(uint32_t val_s, uint32_t row) {
+    double2 v;
+    asm volatile("ld.shared.v2.f64 {%0, %1}, [%2];" : "=d"(v.x), "=d"(v.y) : "r"(val_s + (fu_swz_b(row) & ~15u)));
+    return v;
+}
+__device__ __forceinline__ void fu_sts2(uint32_t val_s, uint32_t row, double2 v) {
+    asm volatile("st.shared.v2.f64 [%0], {%1, %2};" ::"r"(val_s + (fu_swz_b(row) & ~15u)), "d"(v.x), "d"(v.y) : "memory");
+}
+// the accessors of the emit and points loops (not volatile in the order build)
+#if FU_EXP(4)
+__device__ __forceinline__ double fu_lds_o(uint32_t val_s, uint32_t row) {
+    double v;
+    asm("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(val_s + fu_swz_b(row)));
+    return v;
+}
+__device__ __forceinline__ void fu_sts_o(uint32_t val_s, uint32_t row, double v) {
+    asm volatile("st.shared.f64 [%0], %1;" ::"r"(val_s + fu_swz_b(row)), "d"(v));
+}
+__device__ __forceinline__ long long fu_lds_i64_o(uint32_t val_s, uint32_t row) {
+    long long v;
+    asm("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(val_s + fu_swz_b(row)));
+    return v;
+}
+#else
+#define fu_lds_o fu_lds
+#define fu_sts_o fu_sts
+#define fu_lds_i64_o fu_lds_i64
+#endif
 struct FuVals {  // read view for the rollup functions: element i is row r + i
     const double* s;
     uint32_t r;
@@ -507,6 +555,9 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
         FU_PH_COUNT(FU_PH_SERIES);
         FU_PH(FU_PH_SETUP);
 
+#if FU_EXP(1)
+        unsigned long long xacc = 0;  // the folded points of this thread
+#endif
         uint32_t guard = 0;
         while (!bail && (p < P.npoints || !stream_done)) {
             if (++guard > 200000u) {  // every iteration consumes a tile or emits a point: this cannot be reached (the pipeline takes it)
@@ -657,7 +708,11 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                                     const uint32_t u = ((q0 & ~(0xffffffffu << sh)) << cbits) | cval;
                                     const int v32 = (int)((u >> 1) ^ (0u - (u & 1u)));
                                     const long long v = (long long)v32;
+#if FU_EXP(2)
+                                    S.raw32[row - row0][tid] = v32;
+#else
                                     fu_sts_i64(val_s, row, v);  // raw zig-zag decoded delta, replaced by the value in step 4
+#endif
                                     s1 += (uint64_t)v;
                                     s2 += s1;
                                     row++;
@@ -799,14 +854,95 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                         uint32_t cand = 0;  // bit k: row0 + k holds a smaller value than the row in front (a lane has <= 32 rows)
                         const uint64_t v0 = v;
                         const Dec dec = fu_dec(SE);
+                        // the lane's k-th raw delta of the fill
+                        auto fu_emit_raw = [&](uint32_t k) -> uint64_t {
+#if FU_EXP(2)
+                            if (!any_long) return (uint64_t)(int64_t)S.raw32[k & 31u][tid];
+#endif
+                            return (uint64_t)fu_lds_i64_o(val_s, row0 + k);
+                        };
                         auto emit_run = [&](auto is_delta2) {
                             constexpr bool D2 = decltype(is_delta2)::value;
                             // four rows per step: their deltas are loaded first, their conversions are independent of each other and
                             // overlap, their stores come last (row by row, every row waited for its load and for the store in front)
-                            for (uint32_t k = 0; k < cl; k += 4) {
+                            uint32_t k = 0;
+#if FU_EXP(8)
+                            for (; k + 4 <= cl; k += 4) {
                                 uint64_t x[4], vv[4];
 #pragma unroll
-                                for (int i = 0; i < 4; i++) x[i] = (uint64_t)fu_lds_i64(val_s, row0 + k + i);  // (past cl: not used)
+                                for (int i = 0; i < 4; i++) x[i] = fu_emit_raw(k + i);
+#pragma unroll
+                                for (int i = 0; i < 4; i++) {
+                                    if (D2) {
+                                        d1 += x[i];
+                                        v += d1;
+                                    } else {
+                                        v += x[i];
+                                    }
+                                    vv[i] = v;
+                                }
+                                double f[4];
+#pragma unroll
+                                for (int i = 0; i < 4; i++) f[i] = dec.conv_plain((int64_t)vv[i]);
+#pragma unroll
+                                for (int i = 0; i < 4; i++) fu_sts_o(val_s, row0 + k + i, f[i]);
+                            }
+#else
+                            // full batches: no per-row guards, one special-value test for the four rows; the tail (< 4 rows) below
+#if FU_EXP(4)
+                            uint64_t xn[4];
+#pragma unroll
+                            for (int i = 0; i < 4; i++) xn[i] = fu_emit_raw(i);
+#endif
+                            for (; k + 4 <= cl; k += 4) {
+                                uint64_t x[4], vv[4];
+#if FU_EXP(4)
+                                // the next batch's deltas are loaded before this batch's stores (past cl: not used)
+#pragma unroll
+                                for (int i = 0; i < 4; i++) {
+                                    x[i] = xn[i];
+                                    xn[i] = fu_emit_raw(k + 4 + i);
+                                }
+#else
+#pragma unroll
+                                for (int i = 0; i < 4; i++) x[i] = fu_emit_raw(k + i);
+#endif
+                                uint32_t lt = 0;
+#pragma unroll
+                                for (int i = 0; i < 4; i++) {
+                                    const uint64_t pv = v;
+                                    if (D2) {
+                                        d1 += x[i];
+                                        v += d1;
+                                    } else {
+                                        v += x[i];
+                                    }
+                                    lt |= (uint32_t)((int64_t)v < (int64_t)pv) << i;
+                                    vv[i] = v;
+                                }
+                                cand |= lt << k;
+                                double f[4];
+                                bool sp = false;
+#pragma unroll
+                                for (int i = 0; i < 4; i++) {
+                                    f[i] = dec.conv_plain((int64_t)vv[i]);
+                                    sp |= vv[i] - 0x7FFFFFFFFFFFFFFEull < 3ull;  // vStaleNaN / vInfPos / vInfNeg (decimal.go:403-417)
+                                }
+                                if (sp) {
+#pragma unroll
+                                    for (int i = 0; i < 4; i++) {
+                                        f[i] = dec.conv((int64_t)vv[i]);
+                                        saw_stale |= ((int64_t)vv[i] == VMB_V_STALE_NAN);
+                                    }
+                                }
+#pragma unroll
+                                for (int i = 0; i < 4; i++) fu_sts_o(val_s, row0 + k + i, f[i]);
+                            }
+#endif
+                            for (; k < cl; k += 4) {
+                                uint64_t x[4], vv[4];
+#pragma unroll
+                                for (int i = 0; i < 4; i++) x[i] = fu_emit_raw(k + i);  // (past cl: not used)
 #pragma unroll
                                 for (int i = 0; i < 4; i++) {
                                     const uint64_t pv = v;
@@ -831,7 +967,7 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                                             f[i] = dec.conv((int64_t)vv[i]);
                                             saw_stale |= ((int64_t)vv[i] == VMB_V_STALE_NAN);
                                         }
-                                        fu_sts(val_s, row0 + k + i, f[i]);
+                                        fu_sts_o(val_s, row0 + k + i, f[i]);
                                     }
                                 }
                             }
@@ -920,17 +1056,24 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                 const double raw_last = RV[base + cnt - 1];
                 if (nev > FU_MAX_EVENTS) {
                     bail = true;  // a fill full of resets: un-fused path
+                } else if (FU_EXP(16)) {
                 } else if (nev == 0 && corr != 0.0 && isfinite(corr) && fu_ld(S.val, base + cnt_old) + corr >= fu_ld(S.val, base + cnt_old - 1)) {
                     // no value drop inside the fill (nor at its front) and its first corrected row is not below the last output: raw
                     // rows are non-decreasing, x -> RN(x + corr) keeps the order, so the clamp of rollup.go:954 cannot fire: one pass
-                    // (four rows per thread and step, their loads issued before the first store)
-                    for (uint32_t k = cnt_old + tid; k < cnt; k += 4 * FU_THREADS) {
-                        double x[4];
+                    // over 16-byte slot pairs: the swizzle XORs the same value into rows 2m and 2m + 1, so the two share one aligned
+                    // pair of slots (in either order; both get the same correction).  Four pairs per thread and step, their loads
+                    // issued before the first store; a row at either end without its partner in the fill is done on its own.
+                    const uint32_t a0 = base + cnt_old, a1 = base + cnt;
+                    if (tid == 0 && (a0 & 1u)) fu_sts(val_s, a0, fu_lds(val_s, a0) + corr);
+                    if (tid == FU_THREADS - 1 && (a1 & 1u)) fu_sts(val_s, a1 - 1u, fu_lds(val_s, a1 - 1u) + corr);
+                    const uint32_t m1 = a1 >> 1;
+                    for (uint32_t m = ((a0 + 1u) >> 1) + tid; m < m1; m += 4 * FU_THREADS) {
+                        double2 x[4];
 #pragma unroll
-                        for (int i = 0; i < 4; i++) x[i] = fu_lds(val_s, base + k + i * FU_THREADS);  // (past cnt: values not used)
+                        for (int i = 0; i < 4; i++) x[i] = fu_lds2(val_s, 2u * (m + i * FU_THREADS));  // (past m1: values not used)
 #pragma unroll
                         for (int i = 0; i < 4; i++)
-                            if (k + i * FU_THREADS < cnt) fu_sts(val_s, base + k + i * FU_THREADS, x[i] + corr);
+                            if (m + i * FU_THREADS < m1) fu_sts2(val_s, 2u * (m + i * FU_THREADS), make_double2(x[i].x + corr, x[i].y + corr));
                     }
                     FU_PH(FU_PH_RCR);
                     __syncthreads();
@@ -951,37 +1094,72 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                             S.ev_amt[bq + 1] = aa;
                         }
                         double c = corr;
+                        bool fin = isfinite(corr);
                         for (uint32_t a = 0; a < nev; a++) {
                             c = c + S.ev_amt[a];
                             S.ev_cum[a] = c;
+                            fin = fin && isfinite(c);
                         }
+                        // Where can the clamp of rollup.go:954 fire?  Raw rows are never NaN here (a staleness marker hands the
+                        // series to the un-fused path), and a row that is not an event is not below the row in front of it (the
+                        // emit tested every value drop).  With finite corrections x -> RN(x + c) keeps that order, so only the
+                        // fill's first row (against the last output) and the event rows can be below their predecessor: thread 0
+                        // checks those.  Otherwise every row is checked.
+                        uint32_t mode = 1;  // 0: no clamp fires, 1: check every row, 2: a clamp fires
+                        if (fin) {
+                            const uint32_t a0 = base + cnt_old;
+                            const bool ev0 = nev && S.ev_row[0] == a0;
+                            bool viol = !(RV[a0] + (ev0 ? S.ev_cum[0] : corr) >= RV[a0 - 1]);
+                            for (uint32_t a = ev0 ? 1u : 0u; a < nev; a++) {
+                                const uint32_t r = S.ev_row[a];
+                                viol |= !(RV[r] + S.ev_cum[a] >= RV[r - 1] + (a ? S.ev_cum[a - 1] : corr));
+                            }
+                            mode = viol ? 2u : 0u;
+                        }
+                        S.rcr_mode = mode;
                     }
                     FU_PH(FU_PH_RCR);
                     __syncthreads();
                     FU_PH(FU_PH_WAIT);
-                    // corrected values are non-decreasing unless float rounding interferes: check that first, without writing
                     const double prev_out = RV[base + cnt_old - 1];
-                    bool viol = false;
-                    for (uint32_t k = cnt_old + tid; k < cnt; k += FU_THREADS) {
-                        const uint32_t ar = base + k;
-                        double ck = corr, cp = corr;
-                        for (uint32_t a = 0; a < nev; a++) {
-                            if (S.ev_row[a] <= ar) ck = S.ev_cum[a];
-                            if (S.ev_row[a] + 1u <= ar) cp = S.ev_cum[a];
-                        }
-                        const double mk = RV[ar] + ck;
-                        const double mp = k == cnt_old ? prev_out : RV[ar - 1] + cp;
-                        viol |= !(mk >= mp);  // a clamp would fire, or a NaN is involved
-                    }
-                    FU_PH(FU_PH_RCR);
-                    const int any_viol = __syncthreads_or((int)viol);
-                    FU_PH(FU_PH_WAIT);
-                    if (!any_viol) {
+                    const uint32_t mode = S.rcr_mode;
+                    // a thread's rows increase, and so do the events: ck = the correction of the last event at or before the row,
+                    // cp = the same in front of the row (they differ at an event row); one compare per row while no event is passed
+                    uint32_t e = 0, nr = nev ? S.ev_row[0] : 0xffffffffu, lr = 0xffffffffu;
+                    double ck = corr, cq = corr;  // cq: the correction in front of event lr
+                    int any_viol = mode == 2u;
+                    if (mode == 1u) {
+                        // corrected values are non-decreasing unless float rounding interferes: check that first, without writing
+                        bool viol = false;
                         for (uint32_t k = cnt_old + tid; k < cnt; k += FU_THREADS) {
                             const uint32_t ar = base + k;
-                            double ck = corr;
-                            for (uint32_t a = 0; a < nev; a++)
-                                if (S.ev_row[a] <= ar) ck = S.ev_cum[a];
+                            while (nr <= ar) {
+                                cq = ck;
+                                ck = S.ev_cum[e];
+                                lr = nr;
+                                e++;
+                                nr = e < nev ? S.ev_row[e] : 0xffffffffu;
+                            }
+                            const double cp = lr == ar ? cq : ck;
+                            const double mk = RV[ar] + ck;
+                            const double mp = k == cnt_old ? prev_out : RV[ar - 1] + cp;
+                            viol |= !(mk >= mp);  // a clamp would fire, or a NaN is involved
+                        }
+                        FU_PH(FU_PH_RCR);
+                        any_viol = __syncthreads_or((int)viol);
+                        FU_PH(FU_PH_WAIT);
+                    }
+                    if (!any_viol) {
+                        e = 0;
+                        nr = nev ? S.ev_row[0] : 0xffffffffu;
+                        ck = corr;
+                        for (uint32_t k = cnt_old + tid; k < cnt; k += FU_THREADS) {
+                            const uint32_t ar = base + k;
+                            while (nr <= ar) {
+                                ck = S.ev_cum[e];
+                                e++;
+                                nr = e < nev ? S.ev_row[e] : 0xffffffffu;
+                            }
                             RV[ar] = RV[ar] + ck;
                         }
                     } else if (w == 0) {
@@ -1037,7 +1215,11 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                 const bool to_aggr = P.aggr_values != nullptr;
                 double* out_row = P.out + (to_aggr ? (size_t)blockIdx.x : (size_t)SE.s) * P.npoints;
                 asm volatile("" : "+l"(out_row));  // (kept in registers: the loops below are tight)
+#if FU_EXP(1)
+                auto put = [&](uint32_t q, double v) { xacc ^= (unsigned long long)__double_as_longlong(v) + q; };
+#else
                 auto put = [&](uint32_t q, double v) { out_row[q] = v; };
+#endif
                 uint32_t sc_interior = spc ? spc : (uint32_t)rate_rows;  // samplesScanned of an interior rate() point
                 asm volatile("" : "+r"(sc_interior));
                 // a point from its window edges (rate_edges / window_point): every point the interior path below does not take
@@ -1083,14 +1265,34 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                     // interior points: the window [i, j) holds rate_rows rows and row i - 1 exists: (v[j-1] - v[i-1]) / D.  Four points
                     // per thread, their eight edge loads issued before any arithmetic (a point off the range reads ring slots whose
                     // values are not used)
+#if FU_EXP(4)
+                    double np[4], nl[4];  // the edges of the next four points, loaded before this step's stores
+#pragma unroll
+                    for (int k = 0; k < 4; k++) {
+                        const int32_t is_ = iq0 + (int32_t)(p + tid + k * FU_THREADS) * lin_k;
+                        np[k] = fu_lds_o(val_s, (uint32_t)is_ - 1u);
+                        nl[k] = fu_lds_o(val_s, (uint32_t)(is_ + rate_rows) - 1u);
+                    }
+#endif
                     for (uint32_t q = p + tid; q < p_end; q += 4 * FU_THREADS) {
                         double vp[4], vl[4];
+#if FU_EXP(4)
+#pragma unroll
+                        for (int k = 0; k < 4; k++) {
+                            const int32_t is_ = iq0 + (int32_t)(q + (k + 4) * FU_THREADS) * lin_k;
+                            vp[k] = np[k];
+                            vl[k] = nl[k];
+                            np[k] = fu_lds_o(val_s, (uint32_t)is_ - 1u);
+                            nl[k] = fu_lds_o(val_s, (uint32_t)(is_ + rate_rows) - 1u);
+                        }
+#else
 #pragma unroll
                         for (int k = 0; k < 4; k++) {
                             const int32_t is_ = iq0 + (int32_t)(q + k * FU_THREADS) * lin_k;
-                            vp[k] = fu_lds(val_s, (uint32_t)is_ - 1u);
-                            vl[k] = fu_lds(val_s, (uint32_t)(is_ + rate_rows) - 1u);
+                            vp[k] = fu_lds_o(val_s, (uint32_t)is_ - 1u);
+                            vl[k] = fu_lds_o(val_s, (uint32_t)(is_ + rate_rows) - 1u);
                         }
+#endif
                         uint32_t rest = 0;  // points of the four the interior path does not take
 #pragma unroll
                         for (int k = 0; k < 4; k++) {
@@ -1147,6 +1349,10 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
             mbar_wait(&S.mbar[buf], (par >> buf) & 1u);
             par ^= 1u << buf;
         }
+#if FU_EXP(1)
+        if (!bail && tid < P.npoints)
+            P.out[(size_t)(P.aggr_values ? blockIdx.x : SE.s) * P.npoints + tid] = __longlong_as_double((long long)xacc);
+#endif
         if (bail) {
             if (tid == 0) {
                 const unsigned int e = atomicAdd(P.bail_count, 1u);
