@@ -11,6 +11,9 @@ library is left alone -- and each takes one suspect off the per-row loops while 
      4 order     the emit's and the points' shared loads not volatile, the emit's stores without a memory clobber
      8 guards    the emit's full four-row batches without the per-row guards, reset candidates and special-value test
     16 rcr       no counter-reset pass over the rows (the emit still finds the candidates)
+    32 prologue  every series after a CTA's first reuses that series' record (copied in shared memory instead of fetched; only
+                 the output row is its own), its first fill issued one series ahead: what the record fetch costs.  Its
+                 streams are the first series', counter resets included, so the per-CTA work differs from the product's
 The outputs of these builds may be wrong; only their kernel time is read.  Mask 0 is the product library of the tree.  Every
 library runs in its own process over the same generated blocks, the libraries alternate over --rounds, and each process times
 k_fused_rollup (torch.profiler device time, after warm-up) at every grid cap of --caps (CTAs per SM, VMB_FUSED_CTAS_PER_SM; the
@@ -23,7 +26,7 @@ per SM cycle at the maximum SM clock.  --func avg_over_time --kind gauge runs th
 --libs name=path,... alternates more libraries with the builds (a parent's product, say); the result digest (wrapping sums of
 the result's bits over rows and over columns) tells whether two libraries computed the same.
 
-  python scripts/exp_fused_bound.py [--variants 0,1,2,4,8,16] [--caps 3,4,5] [--rounds 2] [--func rate --kind counter]
+  python scripts/exp_fused_bound.py [--variants 0,1,2,4,8,16,32] [--caps 3,4,5] [--rounds 2] [--func rate --kind counter]
                                     [--libs name=path,...] [--prebuilt DIR] [--json out]
 """
 import argparse
@@ -42,7 +45,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "scripts"))
 sys.dont_write_bytecode = True
 
-NAMES = {0: "product", 1: "store", 2: "conflict", 4: "order", 8: "guards", 16: "rcr"}
+NAMES = {0: "product", 1: "store", 2: "conflict", 4: "order", 8: "guards", 16: "rcr", 32: "prologue"}
 SMS = 132
 
 
@@ -136,7 +139,7 @@ def main():
     ap.add_argument("--rows", type=int, default=8192)
     ap.add_argument("--func", default="rate")
     ap.add_argument("--kind", default="counter", help="bench.gen_blocks kind of the generated blocks")
-    ap.add_argument("--variants", default="0,1,2,4,8,16", help="VMB_FUSED_EXP masks (0 = the product library)")
+    ap.add_argument("--variants", default="0,1,2,4,8,16,32", help="VMB_FUSED_EXP masks (0 = the product library)")
     ap.add_argument("--caps", default="3,4,5", help="k_fused_rollup grid caps, CTAs per SM")
     ap.add_argument("--rounds", type=int, default=2, help="alternating rounds over the libraries")
     ap.add_argument("--steps", type=int, default=5, help="profiled calls per cap")

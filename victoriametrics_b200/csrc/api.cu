@@ -67,7 +67,9 @@ struct DevBuf {  // grow-only device buffer
 // ev[ST_FUSED] where the aggregate ends, so stage s spans ev[s] .. ev[s + 1]; eval_fused says which events it records.
 enum Stage { ST_ZSTD, ST_DECODE, ST_PREAMBLE, ST_ROLLUP, ST_AGGR, ST_FUSED, ST__COUNT };
 
-#define FUSED_CHUNKS_DEFAULT 2u /* eval_fused: chunks of the fused series list (VMB_FUSED_CHUNKS overrides) */
+/* eval_fused: chunks of the fused series list (VMB_FUSED_CHUNKS overrides).  1 since the fused CTAs claim their series: they
+   now finish together and leave the zstd stage of a next chunk no room to overlap, so one-shot is faster (DESIGN.md section 8) */
+#define FUSED_CHUNKS_DEFAULT 1u
 #define FUSED_CHUNKS_MAX 64u
 
 struct vmb_ctx {
@@ -81,6 +83,7 @@ struct vmb_ctx {
     DevBuf zseq;  // decoded zstd sequences (8 B each) between k_zstd_seq_decode and k_zstd_seq_exec
     DevBuf zscratch, zlit, zstatus, zjobs, zws, args1, args2, rolled, counters, tmp_out, grp, mheap, mnext;
     DevBuf bail, sub_arrays;  // fused path: series handed to the un-fused pipeline, and that sub-batch's arrays
+    DevBuf fused_recs;        // fused path: one FuSeries record per listed series (k_fused_series_records)
     DevBuf enc_vals, enc_deltas, enc_out, enc_meta;  // vmb_marshal_columns_gpu
     DevBuf aggr_state, grp_ids;  // vmb_eval_rollup_aggr_dist: {values, counts}[G x P]; device copy of the per-series group ids
     // vmb_aggr_order / vmb_transform_range: a batch's keys, its merge buffer, per-cell (per-row) statistics, sort plan
@@ -209,7 +212,7 @@ extern "C" void vmb_ctx_destroy(vmb_ctx* c) {
     if (c->col_cache) vmb_series_free(c->col_cache);
     c->col_cache = nullptr;
     DevBuf* bufs[] = {&c->zscratch, &c->zlit, &c->zstatus, &c->zjobs, &c->zws, &c->args1, &c->args2, &c->rolled,
-                      &c->counters, &c->tmp_out, &c->grp, &c->mheap, &c->mnext, &c->zseq, &c->bail, &c->sub_arrays, &c->aggr_state, &c->grp_ids, &c->enc_vals, &c->enc_deltas, &c->enc_out, &c->enc_meta,
+                      &c->counters, &c->tmp_out, &c->grp, &c->mheap, &c->mnext, &c->zseq, &c->bail, &c->sub_arrays, &c->fused_recs, &c->aggr_state, &c->grp_ids, &c->enc_vals, &c->enc_deltas, &c->enc_out, &c->enc_meta,
                       &c->oa_keys, &c->oa_keys2, &c->oa_cell, &c->oa_meta, &c->cv_runs, &c->cv_aux, &c->cv_uniq};
     for (DevBuf* b : bufs) b->release();
     for (cudaEvent_t e : c->ev)
@@ -1713,6 +1716,7 @@ static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t
     const size_t nf = b->h_fused.size();
     // everything that can fail before any work is forked to zstream
     if ((rc = ctx->bail.reserve((nf + 2) * sizeof(uint32_t)))) return rc;
+    if ((rc = ctx->fused_recs.reserve(nf * sizeof(FuSeries)))) return rc;
     unsigned int* d_bail_count = (unsigned int*)ctx->bail.p;
     uint32_t* d_bail_list = (uint32_t*)ctx->bail.p + 2;
     FusedParams F;
@@ -1734,6 +1738,7 @@ static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t
     F.scanned = c.d_scanned;
     F.bail_list = d_bail_list;
     F.bail_count = d_bail_count;
+    F.claim = d_bail_count + 1;  // (the word between the bail count and the bail list)
     F.npoints = (uint32_t)points;
     F.tr_min = tr_min;
     F.tr_max = tr_max;
@@ -1780,6 +1785,13 @@ static int eval_fused(vmb_ctx* ctx, const vmb_blocks* b, int64_t tr_min, int64_t
         if (k) CU(cudaStreamWaitEvent(st, ctx->zev[k], 0));
         F.ser_list = b->d_fused_list + chunk_begin(k);
         F.nlist = chunk_begin(k + 1) - chunk_begin(k);
+        // the chunk's series records, behind the same zstd stage as its fused launch (the kernel reads nothing else per series)
+        FuSeries* recs = (FuSeries*)ctx->fused_recs.p + chunk_begin(k);
+        F.recs = recs;
+        if (F.nlist) {
+            k_fused_series_records<<<(F.nlist + 127) / 128, 128, 0, st>>>(F, recs);
+            count_launch(ctx);
+        }
         launch_fused(F, ctas_per_sm, st);
         count_launch(ctx);
     }

@@ -90,10 +90,30 @@ __device__ unsigned long long fu_phase_cyc[FU_PH_CTAS][FU_PH_SLOTS];
 //                (software-pipelined; the loads are not volatile and the emit's stores have no memory clobber)
 //    8 guards    the emit's full four-row batches run without the per-row guards, reset candidates and special-value test
 //   16 rcr       no counter-reset pass over the rows (one-pass correction, event path); the emit still finds the candidates
+//   32 prologue  every series after a CTA's first reuses that first series' FuSeries record (only its output row is its own,
+//                its list entry loaded a series ahead), copied in shared memory instead of fetched; its first fill is issued
+//                one series ahead as in the product.  What is left of a series' prologue: the record fetch and its wait
 #ifndef VMB_FUSED_EXP
 #define VMB_FUSED_EXP 0
 #endif
 #define FU_EXP(b) ((VMB_FUSED_EXP & (b)) != 0)
+
+// what one thread of k_fused_series_records derives from the block header and the query for a list entry; the fused kernel
+// fetches it into shared memory with one bulk copy and reads it where it is used
+struct alignas(16) FuSeries {
+    const uint8_t* A;        // 16-byte aligned base of the values stream; stream byte i sits at A[shift + i]
+    int64_t t_org, dts, window, max_prev, dconst, first_value;
+    uint32_t shift, len, n, end_al;
+    int32_t start_r, step32, win32, mpi32;  // the query grid relative to the first row, all below 2^30 in magnitude
+    int32_t lin_k, iq0, jq0;                // step % dt == 0: the window edges of point q are iq0 + q * lin_k, jq0 + q * lin_k
+    double dec_e10, dec_rcp;                // Dec (decimal.go:100) of the block's scale
+    double rate_D, rate_R;                  // rate(): divisor of a full window and its reciprocal (rate_dt = the span in ms, -1: none)
+    int32_t rate_dt, rate_rows, dec_mode;
+    uint32_t s;              // the series (its output row)
+    int16_t scale;
+    uint8_t bail, is_stream, delta2, do_rcr, stale_matters, lin;
+};
+static_assert(sizeof(FuSeries) % 16 == 0, "a record is one cp.async.bulk");
 
 struct FusedParams {
     const vmb_block_desc* descs;
@@ -103,11 +123,13 @@ struct FusedParams {
     const int32_t* zstd_status;      // per column (2*nblocks) or nullptr
     const uint32_t* ser_list;        // series handled by this launch
     const uint32_t* ser_first_block; // per series
+    const FuSeries* recs;            // per list entry (k_fused_series_records)
     vmb_rollup_cfg cfg;              // args / args2: DEVICE pointers
     double* out;                     // [nseries x P]
     unsigned long long* scanned;
     uint32_t* bail_list;             // series this kernel could not finish (-> un-fused pipeline)
     unsigned int* bail_count;
+    unsigned int* claim;             // list entries claimed past each CTA's first two (zeroed by k_fused_series_records)
     uint32_t nlist;
     uint32_t npoints;
     int64_t tr_min, tr_max;
@@ -122,25 +144,10 @@ struct FusedParams {
 
 namespace {
 
-// what one thread derives from the block header and the query for a series (everybody else reads it from shared memory)
-struct FuSeries {
-    const uint8_t* A;        // 16-byte aligned base of the values stream; stream byte i sits at A[shift + i]
-    int64_t t_org, dts, window, max_prev, dconst, first_value;
-    uint32_t shift, len, n, end_al;
-    int32_t start_r, step32, win32, mpi32;  // the query grid relative to the first row, all below 2^30 in magnitude
-    int32_t lin_k, iq0, jq0;                // step % dt == 0: the window edges of point q are iq0 + q * lin_k, jq0 + q * lin_k
-    double dec_e10, dec_rcp;                // Dec (decimal.go:100) of the block's scale
-    double rate_D, rate_R;                  // rate(): divisor of a full window and its reciprocal (rate_dt = the span in ms, -1: none)
-    int32_t rate_dt, rate_rows, dec_mode;
-    uint32_t s;              // the series (its output row)
-    int16_t scale;
-    uint8_t bail, is_stream, delta2, do_rcr, stale_matters, lin;
-};
-
 struct FusedSmem {
     double val[FU_CAP];
     alignas(16) uint8_t stage[2][FU_STAGE];
-    unsigned long long mbar[2];
+    unsigned long long mbar[3];  // the two stage buffers, the record of the next series
     unsigned long long w_s1[FU_WARPS], w_s2[FU_WARPS];
     uint32_t w_cnt[FU_WARPS];
     double ev_amt[FU_MAX_EVENTS], ev_cum[FU_MAX_EVENTS];
@@ -148,12 +155,17 @@ struct FusedSmem {
     uint32_t nev;
     uint32_t rcr_mode;  // how the fill's corrections are applied (thread 0 decides, behind the barrier everybody reads it)
     unsigned long long nd_v, nd_d1;  // nearest-delta(2) state in front of the next fill: last value, last delta
+    uint32_t lnext[2];  // the list entry after the current series (and after the next one), see the series loop
     uint32_t flags;  // bit 0: bail (set while parsing, read behind the barrier that ends the parse)
     uint32_t flags_emit;  // the same for the emit pass: a word of its own, so that a warp already emitting cannot race a warp still reading `flags`
     unsigned long long s_part[FU_WARPS];
     unsigned long long s_thr[FU_THREADS];  // this thread's share of samplesScanned over the series the CTA finished
     unsigned long long s_ser[FU_THREADS];  // the same for the current series (dropped when it is handed to the un-fused path)
     FuSeries ser;  // the current series (read where it is used: it stays valid for the whole series)
+    FuSeries ser_next;  // the next series' record, fetched while the current one finishes
+#if FU_EXP(32)
+    FuSeries ser0;  // the CTA's first series, reused by every later one
+#endif
 #ifdef VMB_FUSED_PHASES
     unsigned long long ph[FU_WARPS][FU_PH_SLOTS];
 #endif
@@ -182,6 +194,17 @@ __device__ __forceinline__ bool mbar_try_wait(unsigned long long* bar, uint32_t 
         : "r"(smem_u32(bar)), "r"(parity)
         : "memory");
     return ok != 0;
+}
+// the spin of a wait that did not succeed at once, out of line (thread 0's wait for the next series' record is made where the
+// fused kernel has no registers to spare); traps like mbar_wait
+__device__ __noinline__ void mbar_wait_slow(unsigned long long* bar, uint32_t parity) {
+    const long long t0 = clock64();
+    while (!mbar_try_wait(bar, parity)) {
+        if (clock64() - t0 > 4000000000LL) {
+            printf("fused: series record did not land (block %u parity %u)\n", blockIdx.x, parity);
+            __trap();
+        }
+    }
 }
 // waits for the phase with the given parity; a copy that never lands (a driver / addressing fault) traps instead of hanging
 __device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t parity) {
@@ -479,13 +502,17 @@ __device__ __forceinline__ void fu_stage_copy(FusedSmem& S, const uint8_t* A, ui
     }
 }
 
-// one thread: series s -> `ser`, and the first fill of its stream (a column the kernel takes) into the idle stage buffer `bf`
-__device__ void fu_series_begin(const FusedParams& P, FusedSmem& S, uint32_t s, FuSeries* ser, uint32_t bf) {
-    fu_series_setup(P, s, ser);
-    if (!ser->bail && ser->is_stream) fu_stage_copy(S, ser->A, ser->end_al, 0, bf);
-}
-
 }  // namespace
+
+// One thread per list entry: the series record k_fused_rollup reads (recs[li] for ser_list[li]).  It runs on the stream right
+// before the fused launch over the same list, so it sees what the zstd stage in front of that launch wrote: the columns'
+// status and the content size of frames without one (set on the device).  Every dependent load of a series' header is made
+// here, in parallel over the series, instead of by one thread of a CTA between two series.
+__global__ void __launch_bounds__(128) k_fused_series_records(FusedParams P, FuSeries* recs) {
+    const uint32_t li = blockIdx.x * blockDim.x + threadIdx.x;
+    if (li == 0) *P.claim = 0;  // (the fused launch over this list runs behind this kernel on the same stream)
+    if (li < P.nlist) fu_series_setup(P, P.ser_list[li], recs + li);
+}
 
 template <int F>
 __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(FusedParams P) {
@@ -497,11 +524,15 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
     const vmb_rollup_cfg& rc = P.cfg;
     const uint32_t tid = threadIdx.x, lane = tid & 31u, w = tid >> 5;
     S.s_thr[tid] = 0;
-    uint32_t par = 0;             // bit b: mbarrier phase parity of stage buffer b (carried over the series)
+    // bit b: mbarrier phase parity of stage buffer b, bit 2: of the record barrier (carried over the series); bits 3-4: the next
+    // series' state, bit 5: which S.lnext slot is the current series' (below; kept here rather than in registers of their own,
+    // which the 96-register budget does not have)
+    uint32_t par = 0;
     uint32_t buf = 0;             // stage buffer of the next tile; a series starts in the one its predecessor left it at
     if (tid == 0) {
         mbar_init(&S.mbar[0], 1);
         mbar_init(&S.mbar[1], 1);
+        mbar_init(&S.mbar[2], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
 #ifdef VMB_FUSED_PHASES
@@ -509,11 +540,62 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
     long long ph_t = clock64();
 #endif
     __syncthreads();
-
-    for (uint32_t li = blockIdx.x; li < P.nlist; li += gridDim.x) {
-        __syncthreads();  // the previous series is done with the shared memory
+    // One series ahead: as soon as the current series needs no more copies, thread 0 fetches the record of the CTA's next list
+    // entry into ser_next (rec_fetch) and, once the record has landed, issues that series' first fill into the idle stage
+    // buffer (first_fill); the current series' last fill and points overlap both.  The loop top falls back to doing both for
+    // the CTA's first series and behind a series that never got there (one that bailed, for instance).
+    // the next series' state: 0 nothing issued, 1 its record in flight, 2 its first fill issued
+    auto nstate = [&]() { return (par >> 3) & 3u; };
+    auto set_nstate = [&](uint32_t v) { par = (par & ~(3u << 3)) | (v << 3); };
+    auto rec_fetch = [&](uint32_t l) {
         if (tid == 0) {
-            fu_series_begin(P, S, P.ser_list[li], &S.ser, buf);
+#if FU_EXP(32)
+            if (l != blockIdx.x) {
+                const uint32_t s = P.ser_list[l];
+                S.ser_next = S.ser0;
+                S.ser_next.s = s;
+                asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&S.mbar[2])) : "memory");
+            } else {
+#endif
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // (thread 0 read ser_next through the generic proxy)
+            mbar_expect_tx(&S.mbar[2], (uint32_t)sizeof(FuSeries));
+            bulk_g2s(&S.ser_next, P.recs + l, (uint32_t)sizeof(FuSeries), &S.mbar[2]);
+#if FU_EXP(32)
+            }
+#endif
+        }
+        set_nstate(1);
+    };
+    auto first_fill = [&](uint32_t bf) {
+        if (tid == 0) {
+            if (!mbar_try_wait(&S.mbar[2], (par >> 2) & 1u)) mbar_wait_slow(&S.mbar[2], (par >> 2) & 1u);
+            if (!S.ser_next.bail && S.ser_next.is_stream) fu_stage_copy(S, S.ser_next.A, S.ser_next.end_al, 0, bf);
+        }
+        par ^= 4u;
+        set_nstate(2);
+    };
+
+    // Series are claimed, not dealt: a CTA runs list entries blockIdx.x and blockIdx.x + gridDim.x, then the entries it claims
+    // from P.claim, so that CTAs whose series cost more run fewer of them and all finish close together.  The claim for the
+    // series after the next is issued at the top of a series and its result is only stored at the series' end (thread 0), so
+    // the atomic's round trip is hidden.  S.lnext[k & 1] holds the entry after the k-th series of the CTA (bit 5 of par: k & 1).
+    if (tid == 0) S.lnext[0] = blockIdx.x + gridDim.x;
+    uint32_t claim = 0;  // thread 0: the claimed entry after the next
+    for (uint32_t li = blockIdx.x; li < P.nlist; li = S.lnext[((par >> 5) & 1u) ^ 1u]) {
+        __syncthreads();  // the previous series is done with the shared memory
+        const uint32_t* const lnext = &S.lnext[(par >> 5) & 1u];  // (read where used: the entry after this series)
+        if (tid == 0 && *lnext < P.nlist) claim = 2 * gridDim.x + atomicAdd(P.claim, 1u);
+        if (nstate() == 0) rec_fetch(li);
+        if (nstate() == 1) first_fill(buf);
+        set_nstate(0);
+        if (tid == 0) {
+            // ser_next -> ser: the record stays where the loops read it for the whole series
+#pragma unroll
+            for (uint32_t k = 0; k < sizeof(FuSeries) / 16; k++)
+                reinterpret_cast<uint4*>(&S.ser)[k] = reinterpret_cast<const uint4*>(&S.ser_next)[k];
+#if FU_EXP(32)
+            if (li == blockIdx.x) S.ser0 = S.ser_next;
+#endif
             S.flags = 0;
             S.flags_emit = 0;
             S.nev = 0;
@@ -533,7 +615,8 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
             if (tid == 0) fu_stage_copy(S, SE.A, SE.end_al, fs, bf);
         };
         uint32_t fs = 0;                   // next unconsumed tile (aligned stream offset); stage[buf] holds it
-        bool copy_pending = !bail && is_stream;  // the first fill is in flight (fu_series_begin)
+        bool copy_pending = !bail && is_stream;  // the first fill is in flight (first_fill)
+        if (!copy_pending && *lnext < P.nlist) rec_fetch(*lnext);  // a series without copies: its successor's record right away
         // first row (nearest_delta2.go:75 / nearest_delta.go:64: as[0] = firstValue)
         uint32_t N = 0;                    // varints decoded so far
         uint32_t base = 0, cnt = 0, p = 0;
@@ -570,6 +653,9 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
             if (is_stream && !stream_done) {
                 FU_PH(FU_PH_POINTS);
                 FU_PH_COUNT(FU_PH_FILLS);
+                // the last fill if all its tiles fit the ring: the next series' record lands while this one is parsed (first_fill
+                // waits until the stream is done: a fill cut short by the ring leaves a copy for this series to come)
+                if (nstate() == 0 && fs + FU_FILL >= SE.end_al && *lnext < P.nlist) rec_fetch(*lnext);
                 if (copy_pending) {
                     mbar_wait(&S.mbar[buf], (par >> buf) & 1u);
                     par ^= 1u << buf;
@@ -1018,6 +1104,7 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                     }
                     __syncthreads();
                     FU_PH(FU_PH_WAIT);
+                    if (nstate() == 1 && stream_done) first_fill(buf);
                     if (tid == 0) {
                         S.nd_v = nV;
                         S.nd_d1 = nD1;
@@ -1367,6 +1454,9 @@ __global__ void __launch_bounds__(FU_THREADS, FU_CTAS_PER_SM) k_fused_rollup(Fus
                 for (uint32_t q = tid; q < P.npoints; q += FU_THREADS) fu_fold(P.aggr_id, P.aggr_values, P.aggr_counts, cell0 + q, row[q]);
             }
         }
+        // the entry after the next (read by everybody behind the barrier at the loop top; nothing reads this slot before it)
+        if (tid == 0) S.lnext[((par >> 5) & 1u) ^ 1u] = *lnext < P.nlist ? claim : P.nlist;
+        par ^= 1u << 5;
         FU_PH(FU_PH_SETUP);
     }
 #ifdef VMB_FUSED_PHASES
