@@ -131,6 +131,17 @@ int vmb_metaindex_row_marshal(uint8_t out[56], const vmb_metaindex_row* row); /*
 int vmb_zstd_decompress_bound(const uint8_t* frames, const uint64_t* offs, size_t n, uint64_t* out_bytes);
 int vmb_zstd_decompress_batch(vmb_ctx* ctx, const uint8_t* frames, const uint64_t* offs, size_t n, uint8_t* dst,
                               size_t dst_cap, uint64_t* dst_offs, uint32_t* dst_lens, int32_t* statuses);
+/* encoding.CompressZSTDLevel (lib/encoding/compress.go:13) for n sources at once on the GPU, host buffers, on the ctx's stream --
+ * the frames of a part's index blocks and metaindex (block_stream_writer.go:121,191).  src + offs[n+1] = the sources back to back,
+ * each 1 byte .. 128 MiB.  Frame i == vmb_zstd_compress(source i), byte for byte.  Frames are written back to back into dst;
+ * dst_offs[n+1] receives their offsets.  dst_cap too small: VMB_ERR_CAP, dst_offs[n] = the bytes needed, dst untouched.
+ * VMB_ERR_INVALID_ARG for an empty or oversized source or a NULL pointer.  n == 0: dst_offs[0] = 0.
+ * Limit (the writer's, shared with vmb_zstd_compress and the marshal paths): a source of 128 KiB < n <= 262143 bytes that compresses
+ * gets ONE Compressed block whose literals regenerate more than Block_Maximum_Size (128 KiB).  The library's decoder accepts that
+ * frame; libzstd and klauspost (blockdec.go:345) reject it.  Index blocks (<= 64 KiB, block_stream_writer.go:152) never reach it;
+ * a metaindex of more than 128 KiB does, so it must not be compressed with this writer. */
+int vmb_zstd_compress_batch(vmb_ctx* ctx, const uint8_t* src, const uint64_t* offs, size_t n, uint8_t* dst, size_t dst_cap,
+                            uint64_t* dst_offs);
 
 /* ---- per-call drop-ins (single column; host buffers; run on the GPU) ------------------------------------- */
 /* encoding.UnmarshalValues / UnmarshalTimestamps  encoding.go:111 / :90 (unmarshalInt64Array :173) */
@@ -144,16 +155,19 @@ int vmb_decimal_to_float(vmb_ctx* ctx, double* dst, const int64_t* va, size_t n,
  * libzstd's output (compressed bytes are unpinned by the reference's tests, SURVEY 8c). */
 int vmb_marshal_int64(uint8_t* dst, size_t cap, size_t* out_len, int* out_mt, int64_t* out_first, const int64_t* vals,
                       size_t n, uint8_t precision_bits);
-/* the library's zstd writer on its own (exposed for tests) */
+/* the library's zstd writer on its own (exposed for tests); see the limit under vmb_zstd_compress_batch */
 int vmb_zstd_compress(uint8_t* dst, size_t cap, size_t* out_len, const uint8_t* src, size_t n);
 /* Block.MarshalData (block.go:192) for ncols equal-length int64 columns on `nthreads` host threads: payloads are written
  * back to back into dst, offs[ncols+1] receives their offsets, mts/firsts the MarshalType and first value of each. */
 int vmb_marshal_columns(uint8_t* dst, size_t cap, uint64_t* offs, uint8_t* mts, int64_t* firsts, const int64_t* vals,
                         size_t ncols, size_t rows, uint8_t precision_bits, int nthreads);
-/* The same with the int64 work on the GPU (csrc/encode.cu): isConst / isDeltaConst / isGauge (encoding.go:289-369) as one pass of warp
+/* The same entirely on the GPU (csrc/encode.cu): isConst / isDeltaConst / isGauge (encoding.go:289-369) as one pass of warp
  * reductions per column, nearest-delta / delta2 (lossless, and the lossy precisionBits < 64 state machine of nearest_delta.go:83),
- * zig-zag varint packing by warp scans; the zstd stage of streams >= 128 bytes and the 0.9 rule (encoding.go:152-167) follow on
- * `nthreads` host threads.  Byte-identical to vmb_marshal_columns.  vals: HOST [ncols x rows]. */
+ * zig-zag varint packing by warp scans; then the zstd stage of streams >= 128 bytes with the library's zstd writer (one CTA per
+ * frame), the 0.9 rule (encoding.go:152-167, type 1 -> 5 / 4 -> 6 where the frame is rejected) and the compaction of the payloads
+ * in column order.  Byte-identical to vmb_marshal_columns (payload, offsets, types, firsts); VMB_ERR_CAP when cap is too small
+ * (offs[ncols] = the bytes needed).  vals: HOST [ncols x rows], rows <= 16384.  nthreads is not read: it only ever chose how many
+ * host threads compressed. */
 int vmb_marshal_columns_gpu(vmb_ctx* ctx, uint8_t* dst, size_t cap, uint64_t* offs, uint8_t* mts, int64_t* firsts,
                             const int64_t* vals, size_t ncols, size_t rows, uint8_t precision_bits, int nthreads);
 /* decimal.AppendFloatToDecimal decimal.go:173 (host-side, write path) */

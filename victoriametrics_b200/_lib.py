@@ -87,6 +87,7 @@ def lib():
         "vmb_metaindex_row_marshal": (C.c_int, [u8p, C.POINTER(MetaindexRow)]),
         "vmb_zstd_decompress_bound": (C.c_int, [u8p, u64p, sz, u64p]),
         "vmb_zstd_decompress_batch": (C.c_int, [vp, u8p, u64p, sz, u8p, sz, u64p, u32p, i32p]),
+        "vmb_zstd_compress_batch": (C.c_int, [vp, u8p, u64p, sz, u8p, sz, u64p]),
         "vmb_calibrate_scale": (C.c_int, [i64p, sz, C.c_int16, i64p, sz, C.c_int16, C.POINTER(C.c_int16)]),
         "vmb_unmarshal_int64": (C.c_int, [vp, i64p, sz, u8p, sz, C.c_int, C.c_int64]),
         "vmb_decimal_to_float": (C.c_int, [vp, f64p, i64p, sz, C.c_int16]),

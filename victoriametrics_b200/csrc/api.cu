@@ -84,7 +84,8 @@ struct vmb_ctx {
     DevBuf zscratch, zlit, zstatus, zjobs, zws, args1, args2, rolled, counters, tmp_out, grp, mheap, mnext;
     DevBuf bail, sub_arrays;  // fused path: series handed to the un-fused pipeline, and that sub-batch's arrays
     DevBuf fused_recs;        // fused path: one FuSeries record per listed series (k_fused_series_records)
-    DevBuf enc_vals, enc_deltas, enc_out, enc_meta;  // vmb_marshal_columns_gpu
+    DevBuf enc_vals, enc_deltas, enc_out, enc_meta;  // vmb_marshal_columns_gpu, vmb_zstd_compress_batch
+    DevBuf enc_frames;                               // ... their compacted payloads
     DevBuf aggr_state, grp_ids;  // vmb_eval_rollup_aggr_dist: {values, counts}[G x P]; device copy of the per-series group ids
     // vmb_aggr_order / vmb_transform_range: a batch's keys, its merge buffer, per-cell (per-row) statistics, sort plan
     DevBuf oa_keys, oa_keys2, oa_cell, oa_meta;
@@ -212,7 +213,7 @@ extern "C" void vmb_ctx_destroy(vmb_ctx* c) {
     if (c->col_cache) vmb_series_free(c->col_cache);
     c->col_cache = nullptr;
     DevBuf* bufs[] = {&c->zscratch, &c->zlit, &c->zstatus, &c->zjobs, &c->zws, &c->args1, &c->args2, &c->rolled,
-                      &c->counters, &c->tmp_out, &c->grp, &c->mheap, &c->mnext, &c->zseq, &c->bail, &c->sub_arrays, &c->fused_recs, &c->aggr_state, &c->grp_ids, &c->enc_vals, &c->enc_deltas, &c->enc_out, &c->enc_meta,
+                      &c->counters, &c->tmp_out, &c->grp, &c->mheap, &c->mnext, &c->zseq, &c->bail, &c->sub_arrays, &c->fused_recs, &c->aggr_state, &c->grp_ids, &c->enc_vals, &c->enc_deltas, &c->enc_out, &c->enc_meta, &c->enc_frames,
                       &c->oa_keys, &c->oa_keys2, &c->oa_cell, &c->oa_meta, &c->cv_runs, &c->cv_aux, &c->cv_uniq};
     for (DevBuf* b : bufs) b->release();
     for (cudaEvent_t e : c->ev)
@@ -1200,6 +1201,61 @@ extern "C" int vmb_zstd_decompress_bound(const uint8_t* frames, const uint64_t* 
     *out_bytes = tot;
     return VMB_OK;
 }
+// encoding.CompressZSTDLevel (compress.go:13) for n sources at once: the library's zstd writer on the GPU (k_zstd_frames,
+// csrc/encode.cu), frame i == vmb_zstd_compress(source i).  Sources up to 128 MiB each, like the decoder's content cap.
+extern "C" int vmb_zstd_compress_batch(vmb_ctx* ctx, const uint8_t* src, const uint64_t* offs, size_t n, uint8_t* dst, size_t dst_cap,
+                                       uint64_t* dst_offs) {
+    if (!ctx || !offs || !dst_offs || n > 0x7fffffffull) return VMB_ERR_INVALID_ARG;
+    if (n == 0) {
+        dst_offs[0] = 0;
+        return VMB_OK;
+    }
+    if (!src || (!dst && dst_cap)) return VMB_ERR_INVALID_ARG;
+    for (size_t i = 0; i < n; i++)
+        if (offs[i + 1] <= offs[i] || offs[i + 1] - offs[i] > kZstdBatchMaxContent) return VMB_ERR_INVALID_ARG;
+    CU(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    const uint64_t total = offs[n] - offs[0];
+    // per source: u64 source offset | u64 frame slot | u32 source bytes | u32 frame bytes; then the frame offsets [n + 1]
+    const size_t o_src = 0, o_slot = o_src + n * 8, o_len = o_slot + n * 8, o_flen = al16(o_len + n * 4), o_out = al16(o_flen + n * 4);
+    std::vector<uint8_t> up(o_flen);
+    uint64_t* soff = (uint64_t*)up.data();
+    uint64_t* slot = (uint64_t*)(up.data() + o_slot);
+    uint32_t* len = (uint32_t*)(up.data() + o_len);
+    uint64_t so = al16(total);
+    for (size_t i = 0; i < n; i++) {
+        soff[i] = offs[i] - offs[0];
+        len[i] = (uint32_t)(offs[i + 1] - offs[i]);
+        slot[i] = so;
+        so += al16(zw::raw_frame_len(len[i], 9));
+    }
+    int rc;
+    if ((rc = ctx->enc_meta.reserve(al16(o_out + (n + 1) * 8) + 64))) return rc;
+    if ((rc = ctx->enc_out.reserve(so + 64))) return rc;
+    if ((rc = ctx->enc_frames.reserve(so - al16(total) + 64))) return rc;
+    uint8_t* dm = (uint8_t*)ctx->enc_meta.p;
+    CU(cudaMemcpyAsync(ctx->enc_out.p, src + offs[0], total, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(dm, up.data(), up.size(), cudaMemcpyHostToDevice, st));
+    ZstdFrameJobs J;
+    J.base = (uint8_t*)ctx->enc_out.p;
+    J.src_off = (const uint64_t*)(dm + o_src);
+    J.len = (const uint32_t*)(dm + o_len);
+    J.slot_off = (const uint64_t*)(dm + o_slot);
+    J.frame_len = (uint32_t*)(dm + o_flen);
+    J.n = (uint32_t)n;
+    uint64_t* d_out = (uint64_t*)(dm + o_out);
+    launch_zstd_frames(J, st);
+    launch_scan_lens(J.frame_len, d_out, (uint32_t)n, st);
+    launch_compact(J.base, J.slot_off, d_out, (uint8_t*)ctx->enc_frames.p, (uint32_t)n, st);
+    count_launch(ctx, 3);
+    CU(cudaMemcpyAsync(dst_offs, d_out, (n + 1) * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    if (dst_offs[n] > dst_cap) return VMB_ERR_CAP;
+    CU(cudaMemcpyAsync(dst, ctx->enc_frames.p, dst_offs[n], cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    return VMB_OK;
+}
 extern "C" int vmb_zstd_decompress_batch(vmb_ctx* ctx, const uint8_t* frames, const uint64_t* offs, size_t n, uint8_t* dst,
                                          size_t dst_cap, uint64_t* dst_offs, uint32_t* dst_lens, int32_t* statuses) {
     if (!ctx || !frames || !offs || !dst_offs || !dst_lens || n == 0 || n > 0x7fffffffull) return VMB_ERR_INVALID_ARG;
@@ -1964,10 +2020,10 @@ extern "C" int vmb_marshal_columns(uint8_t* dst, size_t cap, uint64_t* offs, uin
     return VMB_OK;
 }
 
-// Block.MarshalData (block.go:192) for many equal-length columns with the int64 work on the GPU (csrc/encode.cu): type detection,
-// nearest-delta / delta2 (lossless and lossy precisionBits), zig-zag varint packing; the zstd stage of streams >= 128 bytes and the
-// 0.9 rule (encoding.go:152-167) follow on `nthreads` host threads with the library's zstd writer.  Same output layout and the same
-// bytes as vmb_marshal_columns.
+// Block.MarshalData (block.go:192) for many equal-length columns entirely on the GPU (csrc/encode.cu): type detection,
+// nearest-delta / delta2 (lossless and lossy precisionBits), zig-zag varint packing, then the zstd stage of streams >= 128 bytes
+// with the library's zstd writer (k_zstd_frames), the 0.9 rule (encoding.go:152-167) and the compaction of the payloads in column
+// order.  Same output layout and the same bytes as vmb_marshal_columns; `nthreads` is not read.
 extern "C" int vmb_marshal_columns_gpu(vmb_ctx* ctx, uint8_t* dst, size_t cap, uint64_t* offs, uint8_t* mts, int64_t* firsts,
                                        const int64_t* vals, size_t ncols, size_t rows, uint8_t precision_bits, int nthreads) {
     if (!ctx || !dst || !offs || !mts || !firsts || !vals || rows == 0 || rows > 16384 || ncols > 0x7fffffffu || precision_bits < 1 ||
@@ -1982,9 +2038,12 @@ extern "C" int vmb_marshal_columns_gpu(vmb_ctx* ctx, uint8_t* dst, size_t cap, u
     int rc;
     const size_t nvals = ncols * rows;
     if ((rc = ctx->enc_vals.reserve(nvals * 8))) return rc;
-    // per column: u32 size | u8 mt (padded to 4) | i64 first | u64 offset
-    const size_t o_sizes = 0, o_mts = al16(o_sizes + ncols * 4), o_firsts = al16(o_mts + ncols), o_offs = al16(o_firsts + ncols * 8);
-    if ((rc = ctx->enc_meta.reserve(al16(o_offs + ncols * 8) + 64))) return rc;
+    // per column: u32 size | u8 mt | i64 first | u64 stream offset | u64 frame slot | u32 zstd source bytes | u32 frame bytes |
+    // u64 payload source | u32 payload bytes; then the payload offsets [ncols + 1]
+    const size_t o_sizes = 0, o_mts = al16(o_sizes + ncols * 4), o_firsts = al16(o_mts + ncols), o_offs = al16(o_firsts + ncols * 8),
+                 o_slot = o_offs + ncols * 8, o_zlen = o_slot + ncols * 8, o_flen = al16(o_zlen + ncols * 4),
+                 o_csrc = al16(o_flen + ncols * 4), o_clen = al16(o_csrc + ncols * 8), o_out = al16(o_clen + ncols * 4);
+    if ((rc = ctx->enc_meta.reserve(al16(o_out + (ncols + 1) * 8) + 64))) return rc;
     const bool may_be_lossy = precision_bits < 64;
     if (may_be_lossy && (rc = ctx->enc_deltas.reserve(nvals * 8))) return rc;
     CU(cudaMemcpyAsync(ctx->enc_vals.p, vals, nvals * 8, cudaMemcpyHostToDevice, st));
@@ -2008,55 +2067,52 @@ extern "C" int vmb_marshal_columns_gpu(vmb_ctx* ctx, uint8_t* dst, size_t cap, u
     CU(cudaMemcpyAsync(pmts.data(), M.mts, ncols, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(firsts, M.firsts, ncols * 8, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    std::vector<uint64_t> soffs(ncols + 1, 0);
-    for (size_t c = 0; c < ncols; c++) soffs[c + 1] = soffs[c] + sizes[c];
-    const uint64_t total = soffs[ncols];
-    if ((rc = ctx->enc_out.reserve(total + 64))) return rc;
-    CU(cudaMemcpyAsync(dm + o_offs, soffs.data(), ncols * 8, cudaMemcpyHostToDevice, st));
+    // streams back to back, then a frame slot for each stream of type 1 / 4 of >= 128 bytes (encoding.go:152)
+    std::vector<uint8_t> up(o_flen - o_offs);
+    uint64_t* soffs = (uint64_t*)up.data();
+    uint64_t* slot = (uint64_t*)(up.data() + (o_slot - o_offs));
+    uint32_t* zlen = (uint32_t*)(up.data() + (o_zlen - o_offs));
+    uint64_t total = 0;
+    for (size_t c = 0; c < ncols; c++) {
+        soffs[c] = total;
+        total += sizes[c];
+    }
+    const size_t min_compressible = 128;  // encoding.go:15
+    uint64_t so = al16(total);
+    for (size_t c = 0; c < ncols; c++) {
+        zlen[c] = (pmts[c] == 1 || pmts[c] == 4) && sizes[c] >= min_compressible ? sizes[c] : 0;
+        slot[c] = so;
+        so += zlen[c] ? al16(zw::raw_frame_len(zlen[c], 9)) : 0;
+    }
+    if ((rc = ctx->enc_out.reserve(so + 64))) return rc;
+    if ((rc = ctx->enc_frames.reserve(total + 64))) return rc;  // a frame is kept only when smaller than its stream
+    CU(cudaMemcpyAsync(dm + o_offs, up.data(), up.size(), cudaMemcpyHostToDevice, st));
     M.out = (uint8_t*)ctx->enc_out.p;
     launch_marshal_pack(M, st);
-    count_launch(ctx);
-    std::vector<uint8_t> streams(total + 1);
-    if (total) CU(cudaMemcpyAsync(streams.data(), M.out, total, cudaMemcpyDeviceToHost, st));
+    ZstdFrameJobs J;
+    J.base = (uint8_t*)ctx->enc_out.p;
+    J.src_off = (const uint64_t*)(dm + o_offs);
+    J.len = (const uint32_t*)(dm + o_zlen);
+    J.slot_off = (const uint64_t*)(dm + o_slot);
+    J.frame_len = (uint32_t*)(dm + o_flen);
+    J.n = (uint32_t)ncols;
+    launch_zstd_frames(J, st);
+    uint64_t* d_csrc = (uint64_t*)(dm + o_csrc);
+    uint32_t* d_clen = (uint32_t*)(dm + o_clen);
+    uint64_t* d_out = (uint64_t*)(dm + o_out);
+    launch_marshal_select(M.sizes, J.src_off, J, M.mts, d_csrc, d_clen, (uint32_t)ncols, st);
+    launch_scan_lens(d_clen, d_out, (uint32_t)ncols, st);
+    launch_compact(J.base, d_csrc, d_out, (uint8_t*)ctx->enc_frames.p, (uint32_t)ncols, st);
+    count_launch(ctx, 5);
+    CU(cudaMemcpyAsync(offs, d_out, (ncols + 1) * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(mts, M.mts, ncols, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
-    // ---- zstd stage + the 0.9 rule on host threads
-    std::vector<std::vector<uint8_t>> outs(ncols);
-    std::atomic<size_t> next{0};
-    auto worker = [&]() {
-        for (;;) {
-            const size_t c = next.fetch_add(1);
-            if (c >= ncols) break;
-            const uint8_t* bb = streams.data() + soffs[c];
-            const size_t blen = sizes[c];
-            uint8_t mt = pmts[c];
-            if (mt == 1 || mt == 4) {
-                const size_t min_compressible = 128;  // encoding.go:15
-                if (blen >= min_compressible) vmb_host::zstd_compress_huf(outs[c], bb, blen);
-                if (blen < min_compressible || (double)outs[c].size() > 0.9 * (double)blen) {  // encoding.go:156
-                    mt = mt == 1 ? 5 : 6;
-                    outs[c].assign(bb, bb + blen);
-                }
-            } else {
-                outs[c].assign(bb, bb + blen);
-            }
-            mts[c] = mt;
-        }
-    };
-    if (nthreads <= 1) worker();
-    else {
-        std::vector<std::thread> th;
-        for (int t = 0; t < nthreads; t++) th.emplace_back(worker);
-        for (auto& t : th) t.join();
+    if (offs[ncols] > cap) return VMB_ERR_CAP;
+    if (offs[ncols]) {
+        CU(cudaMemcpyAsync(dst, ctx->enc_frames.p, offs[ncols], cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
     }
-    uint64_t o = 0;
-    for (size_t c = 0; c < ncols; c++) {
-        offs[c] = o;
-        if (o + outs[c].size() > cap) return VMB_ERR_CAP;
-        if (!outs[c].empty()) memcpy(dst + o, outs[c].data(), outs[c].size());
-        o += outs[c].size();
-    }
-    offs[ncols] = o;
     return VMB_OK;
 }
 

@@ -54,6 +54,28 @@ def zstd_compress(src):
     return dst[:n.value].copy()
 
 
+def zstd_compress_batch(sources, ctx=None):
+    """encoding.CompressZSTDLevel compress.go:13 for a list of sources at once (GPU) -> list of np.uint8 frames, each equal to
+    zstd_compress(source) byte for byte.  Every source needs 1 byte .. 128 MiB."""
+    ctx = ctx or _lib.default_context()
+    srcs = [np.ascontiguousarray(np.frombuffer(s, dtype=np.uint8) if isinstance(s, (bytes, bytearray)) else s, dtype=np.uint8)
+            for s in sources]
+    n = len(srcs)
+    if n == 0:
+        return []
+    offs = np.zeros(n + 1, dtype=np.uint64)
+    offs[1:] = np.cumsum([s.size for s in srcs])
+    arena = np.concatenate(srcs)
+    if arena.size == 0:
+        arena = np.zeros(1, dtype=np.uint8)
+    # the writer never makes a frame larger than the Raw-block frame: header + source + a 3-byte header per 128 KiB
+    dst = np.empty(int(offs[-1]) + n * 9 + 3 * sum(-(-s.size // (1 << 17)) for s in srcs), dtype=np.uint8)
+    doffs = np.zeros(n + 1, dtype=np.uint64)
+    check(lib().vmb_zstd_compress_batch(ctx.h, arena.ctypes.data_as(_lib.u8p), offs.ctypes.data_as(_lib.u64p), n,
+                                        dst.ctypes.data_as(_lib.u8p), dst.size, doffs.ctypes.data_as(_lib.u64p)))
+    return [dst[int(doffs[i]):int(doffs[i + 1])].copy() for i in range(n)]
+
+
 def decompress_zstd_batch(frames, ctx=None):
     """encoding.DecompressZSTD compress.go:27 for a list of frames at once (GPU) -> list of np.uint8 arrays.
     Raises VmbError(VMB_ERR_ZSTD) if a frame is corrupt, like the Go error return."""
@@ -83,8 +105,9 @@ def decompress_zstd_batch(frames, ctx=None):
 def marshal_columns(vals2d, precision_bits=64, nthreads=None, ctx=None):
     """batched MarshalValues for equal-length columns: vals2d [ncols x rows] int64
     -> (payload np.uint8, offs np.uint64[ncols+1], mts np.uint8[ncols], firsts np.int64[ncols]).
-    ctx given: type detection, delta coding and varint packing run on the GPU (vmb_marshal_columns_gpu, csrc/encode.cu), the zstd
-    stage on host threads; the bytes are the same either way."""
+    ctx given: everything runs on the GPU (vmb_marshal_columns_gpu, csrc/encode.cu) -- type detection, delta coding, varint
+    packing, the zstd stage with the 0.9 rule, and the compaction of the payloads; nthreads is then not used.  Without ctx,
+    nthreads host threads do the work.  The bytes are the same either way."""
     import os
     a = np.ascontiguousarray(vals2d, dtype=np.int64)
     ncols, rows = a.shape
