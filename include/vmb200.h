@@ -143,6 +143,41 @@ int vmb_zstd_decompress_batch(vmb_ctx* ctx, const uint8_t* frames, const uint64_
 int vmb_zstd_compress_batch(vmb_ctx* ctx, const uint8_t* src, const uint64_t* offs, size_t n, uint8_t* dst, size_t dst_cap,
                             uint64_t* dst_offs);
 
+/* ---- part merges  ==  mergeBlockStreams (lib/storage/merge.go:19) + blockStreamWriter (block_stream_writer.go) ----------------- */
+typedef struct {  /* the four data files of a part directory (part.go:34), host buffers */
+    const uint8_t *metaindex, *index, *timestamps, *values;
+    uint64_t metaindex_len, index_len, timestamps_len, values_len;
+} vmb_part_files;
+typedef struct {
+    uint64_t rows_count, blocks_count; /* partHeader after the merge; min_ts / max_ts = INT64_MAX / INT64_MIN when nothing is left */
+    int64_t min_ts, max_ts;
+    uint64_t rows_merged, rows_deleted; /* the rowsMerged / rowsDeleted counters of mergeBlockStreams */
+} vmb_merge_stats;
+typedef struct vmb_merged_part vmb_merged_part;
+/* Merges parts[0..nparts) in that order (blockStreamMerger's heap and its ties: block_stream_merger.go) into one part, byte for byte
+ * what mergeBlockStreams writes with the library's zstd writer in place of CompressZSTDLevel:
+ *   - blocks of deleted_metric_ids (sorted ascending, unique; VMB_ERR_INVALID_ARG otherwise) and blocks with MaxTimestamp <
+ *     retention_deadline are dropped, rows before the deadline inside merged blocks too (all counted in rows_deleted);
+ *   - blocks of one MetricID are merged by the pending-block chain of merge.go:65-156 (CalibrateScale, PrecisionBits = min,
+ *     mergeBlocks, the split at 8192 rows); a block the chain never unmarshals keeps its payload bytes as they are;
+ *   - the ctx's dedup interval (vmb_ctx_set_dedup_interval) > 0: deduplicateSamplesDuringMerge (dedup.go:94) on every block;
+ *   - identical consecutive timestamps payloads are stored once, index blocks hold at most 809 headers, one metaindex frame.
+ * Every frame is accepted by libzstd: a column stream of 128 KiB < n <= 262143 bytes gets no frame of the writer (MarshalType 1 -> 5,
+ * 4 -> 6), a metaindex of that size (or an empty one) goes into a frame of Raw blocks.  A re-encoded column whose payload exceeds
+ * 128 KiB (such a stream uncompressed; blockHeader.validate block_header.go:248 rejects it) fails the merge with VMB_ERR_CAP.  A part whose metaindex decodes to 0 bytes
+ * is an empty part.  Errors: offsets outside a file (VMB_ERR_SHORT_SRC), a header or metaindex row that fails validation, a block
+ * the merge must unmarshal that fails to decode (its VMB_ERR_* code); *out is then NULL.  Device memory for the whole merge is
+ * needed at once (VMB_ERR_NOMEM otherwise): about 64 bytes per row of every block the merge may unmarshal (the decoded rows and
+ * the chain's three regions), plus the payloads and the encoder's scratch. */
+int vmb_merge_parts(vmb_ctx* ctx, const vmb_part_files* parts, size_t nparts, int64_t retention_deadline,
+                    const uint64_t* deleted_metric_ids, size_t ndeleted, vmb_merged_part** out, vmb_merge_stats* stats);
+/* the metaindex frame vmb_merge_parts writes for an n-byte metaindex (exposed for tests): the library's zstd writer, a frame of Raw
+ * blocks for n == 0 and 128 KiB < n <= 262143.  *out_len = the frame's length (also with VMB_ERR_CAP when cap is too small). */
+int vmb_merge_metaindex_frame(vmb_ctx* ctx, const uint8_t* src, size_t n, uint8_t* dst, size_t cap, size_t* out_len);
+/* the merged part's files: pointers into the part's pinned host memory, valid until vmb_merged_part_free */
+int vmb_merged_part_files(const vmb_merged_part* p, vmb_part_files* files);
+void vmb_merged_part_free(vmb_merged_part* p);
+
 /* ---- per-call drop-ins (single column; host buffers; run on the GPU) ------------------------------------- */
 /* encoding.UnmarshalValues / UnmarshalTimestamps  encoding.go:111 / :90 (unmarshalInt64Array :173) */
 int vmb_unmarshal_int64(vmb_ctx* ctx, int64_t* dst, size_t items_count, const uint8_t* src, size_t src_len, int mt,

@@ -33,6 +33,18 @@ class MetaindexRow(C.Structure):
 assert C.sizeof(MetaindexRow) == 56
 
 
+class PartFiles(C.Structure):
+    """vmb_part_files: the four data files of a part (lib/storage/part.go:34)"""
+    _fields_ = [("metaindex", u8p), ("index", u8p), ("timestamps", u8p), ("values", u8p), ("metaindex_len", C.c_uint64),
+                ("index_len", C.c_uint64), ("timestamps_len", C.c_uint64), ("values_len", C.c_uint64)]
+
+
+class MergeStats(C.Structure):
+    """vmb_merge_stats: partHeader after the merge + the rowsMerged / rowsDeleted counters"""
+    _fields_ = [("rows_count", C.c_uint64), ("blocks_count", C.c_uint64), ("min_ts", C.c_int64), ("max_ts", C.c_int64),
+                ("rows_merged", C.c_uint64), ("rows_deleted", C.c_uint64)]
+
+
 class RollupCfg(C.Structure):
     """vmb_rollup_cfg == rollupConfig (rollup.go:574)"""
     _fields_ = [("func_id", C.c_int32), ("flags", C.c_uint32), ("start", C.c_int64), ("end", C.c_int64),
@@ -88,6 +100,10 @@ def lib():
         "vmb_zstd_decompress_bound": (C.c_int, [u8p, u64p, sz, u64p]),
         "vmb_zstd_decompress_batch": (C.c_int, [vp, u8p, u64p, sz, u8p, sz, u64p, u32p, i32p]),
         "vmb_zstd_compress_batch": (C.c_int, [vp, u8p, u64p, sz, u8p, sz, u64p]),
+        "vmb_merge_parts": (C.c_int, [vp, C.POINTER(PartFiles), sz, C.c_int64, u64p, sz, C.POINTER(vp), C.POINTER(MergeStats)]),
+        "vmb_merged_part_files": (C.c_int, [vp, C.POINTER(PartFiles)]),
+        "vmb_merged_part_free": (None, [vp]),
+        "vmb_merge_metaindex_frame": (C.c_int, [vp, u8p, sz, u8p, sz, C.POINTER(sz)]),
         "vmb_calibrate_scale": (C.c_int, [i64p, sz, C.c_int16, i64p, sz, C.c_int16, C.POINTER(C.c_int16)]),
         "vmb_unmarshal_int64": (C.c_int, [vp, i64p, sz, u8p, sz, C.c_int, C.c_int64]),
         "vmb_decimal_to_float": (C.c_int, [vp, f64p, i64p, sz, C.c_int16]),

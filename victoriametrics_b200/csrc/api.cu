@@ -2024,41 +2024,26 @@ extern "C" int vmb_marshal_columns(uint8_t* dst, size_t cap, uint64_t* offs, uin
 // nearest-delta / delta2 (lossless and lossy precisionBits), zig-zag varint packing, then the zstd stage of streams >= 128 bytes
 // with the library's zstd writer (k_zstd_frames), the 0.9 rule (encoding.go:152-167) and the compaction of the payloads in column
 // order.  Same output layout and the same bytes as vmb_marshal_columns; `nthreads` is not read.
-extern "C" int vmb_marshal_columns_gpu(vmb_ctx* ctx, uint8_t* dst, size_t cap, uint64_t* offs, uint8_t* mts, int64_t* firsts,
-                                       const int64_t* vals, size_t ncols, size_t rows, uint8_t precision_bits, int nthreads) {
-    if (!ctx || !dst || !offs || !mts || !firsts || !vals || rows == 0 || rows > 16384 || ncols > 0x7fffffffu || precision_bits < 1 ||
-        precision_bits > 64)
-        return VMB_ERR_INVALID_ARG;
-    CU(cudaSetDevice(ctx->device));
+// The stages of vmb_marshal_columns_gpu once the values are on the device (M.vals, M.deltas, M.pb or M.col_*; M.ncols): plan, pack,
+// the zstd frames, the 0.9 rule and the compaction of the payloads into ctx->enc_frames; *d_offs receives the device copy of offs.
+// offs [ncols + 1], mts, firsts: HOST.  skip_mid: streams of 128 KiB < n <= 262143 bytes get no frame (so they stay uncompressed,
+// MarshalType 1 -> 5 / 4 -> 6): the writer's single Compressed block for such a source is rejected by libzstd (vmb200.h).
+static int marshal_columns_dev(vmb_ctx* ctx, MarshalParams& M, uint64_t* offs, uint8_t* mts, int64_t* firsts, bool skip_mid,
+                               const uint64_t** d_offs) {
     cudaStream_t st = ctx->stream;
-    if (ncols == 0) {
-        offs[0] = 0;
-        return VMB_OK;
-    }
+    const size_t ncols = M.ncols;
     int rc;
-    const size_t nvals = ncols * rows;
-    if ((rc = ctx->enc_vals.reserve(nvals * 8))) return rc;
     // per column: u32 size | u8 mt | i64 first | u64 stream offset | u64 frame slot | u32 zstd source bytes | u32 frame bytes |
     // u64 payload source | u32 payload bytes; then the payload offsets [ncols + 1]
     const size_t o_sizes = 0, o_mts = al16(o_sizes + ncols * 4), o_firsts = al16(o_mts + ncols), o_offs = al16(o_firsts + ncols * 8),
                  o_slot = o_offs + ncols * 8, o_zlen = o_slot + ncols * 8, o_flen = al16(o_zlen + ncols * 4),
                  o_csrc = al16(o_flen + ncols * 4), o_clen = al16(o_csrc + ncols * 8), o_out = al16(o_clen + ncols * 4);
     if ((rc = ctx->enc_meta.reserve(al16(o_out + (ncols + 1) * 8) + 64))) return rc;
-    const bool may_be_lossy = precision_bits < 64;
-    if (may_be_lossy && (rc = ctx->enc_deltas.reserve(nvals * 8))) return rc;
-    CU(cudaMemcpyAsync(ctx->enc_vals.p, vals, nvals * 8, cudaMemcpyHostToDevice, st));
     uint8_t* dm = (uint8_t*)ctx->enc_meta.p;
-    MarshalParams M;
-    memset(&M, 0, sizeof(M));
-    M.vals = (const int64_t*)ctx->enc_vals.p;
-    M.deltas = may_be_lossy ? (int64_t*)ctx->enc_deltas.p : nullptr;
     M.sizes = (uint32_t*)(dm + o_sizes);
     M.mts = dm + o_mts;
     M.firsts = (int64_t*)(dm + o_firsts);
     M.offs = (const uint64_t*)(dm + o_offs);
-    M.ncols = (uint32_t)ncols;
-    M.rows = (uint32_t)rows;
-    M.pb = precision_bits;
     launch_marshal_plan(M, st);
     count_launch(ctx);
     std::vector<uint32_t> sizes(ncols);
@@ -2081,6 +2066,7 @@ extern "C" int vmb_marshal_columns_gpu(vmb_ctx* ctx, uint8_t* dst, size_t cap, u
     uint64_t so = al16(total);
     for (size_t c = 0; c < ncols; c++) {
         zlen[c] = (pmts[c] == 1 || pmts[c] == 4) && sizes[c] >= min_compressible ? sizes[c] : 0;
+        if (skip_mid && zlen[c] > zw::kMaxBlock && zlen[c] < 262144u) zlen[c] = 0;
         slot[c] = so;
         so += zlen[c] ? al16(zw::raw_frame_len(zlen[c], 9)) : 0;
     }
@@ -2108,6 +2094,35 @@ extern "C" int vmb_marshal_columns_gpu(vmb_ctx* ctx, uint8_t* dst, size_t cap, u
     CU(cudaMemcpyAsync(mts, M.mts, ncols, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
+    if (d_offs) *d_offs = d_out;
+    return VMB_OK;
+}
+
+extern "C" int vmb_marshal_columns_gpu(vmb_ctx* ctx, uint8_t* dst, size_t cap, uint64_t* offs, uint8_t* mts, int64_t* firsts,
+                                       const int64_t* vals, size_t ncols, size_t rows, uint8_t precision_bits, int nthreads) {
+    if (!ctx || !dst || !offs || !mts || !firsts || !vals || rows == 0 || rows > 16384 || ncols > 0x7fffffffu || precision_bits < 1 ||
+        precision_bits > 64)
+        return VMB_ERR_INVALID_ARG;
+    CU(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    if (ncols == 0) {
+        offs[0] = 0;
+        return VMB_OK;
+    }
+    int rc;
+    const size_t nvals = ncols * rows;
+    if ((rc = ctx->enc_vals.reserve(nvals * 8))) return rc;
+    const bool may_be_lossy = precision_bits < 64;
+    if (may_be_lossy && (rc = ctx->enc_deltas.reserve(nvals * 8))) return rc;
+    CU(cudaMemcpyAsync(ctx->enc_vals.p, vals, nvals * 8, cudaMemcpyHostToDevice, st));
+    MarshalParams M;
+    memset(&M, 0, sizeof(M));
+    M.vals = (const int64_t*)ctx->enc_vals.p;
+    M.deltas = may_be_lossy ? (int64_t*)ctx->enc_deltas.p : nullptr;
+    M.ncols = (uint32_t)ncols;
+    M.rows = (uint32_t)rows;
+    M.pb = precision_bits;
+    if ((rc = marshal_columns_dev(ctx, M, offs, mts, firsts, false, nullptr))) return rc;
     if (offs[ncols] > cap) return VMB_ERR_CAP;
     if (offs[ncols]) {
         CU(cudaMemcpyAsync(dst, ctx->enc_frames.p, offs[ncols], cudaMemcpyDeviceToHost, st));
@@ -2143,3 +2158,4 @@ extern "C" int vmb_float_to_decimal_columns(vmb_ctx* ctx, int64_t* dst, int16_t*
     CU(cudaGetLastError());
     return VMB_OK;
 }
+#include "merge.inc"

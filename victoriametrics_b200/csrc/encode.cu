@@ -30,6 +30,11 @@ struct MarshalParams {
     int64_t* firsts;          // [ncols]
     uint32_t ncols, rows;
     uint32_t pb;              // precisionBits 1..64
+    // ragged columns (the merge path): column c holds col_rows[c] values at vals + col_off[c] with precisionBits col_pb[c];
+    // nullptr: every column holds `rows` values at c * rows with precisionBits pb
+    const uint64_t* col_off;
+    const uint32_t* col_rows;
+    const uint8_t* col_pb;
 };
 
 namespace {
@@ -73,14 +78,29 @@ __device__ __forceinline__ int64_t enc_stream_value(const int64_t* a, const int6
     return (int64_t)((uint64_t)a[i] - 2ull * (uint64_t)a[i - 1] + (uint64_t)a[i - 2]);  // next - v - d1, nearest_delta2.go:30
 }
 
+// where column c lives, how many values it holds and at which precisionBits it is written
+__device__ __forceinline__ void enc_col(const MarshalParams& P, uint32_t c, uint64_t* off, uint32_t* n, uint32_t* pb) {
+    if (P.col_off) {
+        *off = P.col_off[c];
+        *n = P.col_rows[c];
+        *pb = P.col_pb[c];
+    } else {
+        *off = (uint64_t)c * P.rows;
+        *n = P.rows;
+        *pb = P.pb;
+    }
+}
+
 }  // namespace
 
 __global__ void __launch_bounds__(128) k_marshal_plan(MarshalParams P) {
     const int lane = lane_id();
     const uint32_t wpg = gridDim.x * (blockDim.x >> 5);
     for (uint32_t c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < P.ncols; c += wpg) {
-        const int64_t* a = P.vals + (size_t)c * P.rows;
-        const uint32_t n = P.rows;
+        uint64_t co;
+        uint32_t n, cpb;
+        enc_col(P, c, &co, &n, &cpb);
+        const int64_t* a = P.vals + co;
         const int64_t a0 = a[0];
         // ---- detection: isConst, isDeltaConst, isGauge in one pass
         const uint64_t d1 = n >= 2 ? (uint64_t)a[1] - (uint64_t)a0 : 0ull;
@@ -110,10 +130,10 @@ __global__ void __launch_bounds__(128) k_marshal_plan(MarshalParams P) {
         } else {
             mt = gauge ? 4u : 1u;
             const bool delta2 = !gauge;
-            uint32_t pb = P.pb;
+            uint32_t pb = cpb;
             if (gauge && pb < 6) pb += 2;                        // encoding.go:141
             const bool lossy = pb < 64;
-            int64_t* dl = lossy ? P.deltas + (size_t)c * P.rows : nullptr;
+            int64_t* dl = lossy ? P.deltas + co : nullptr;
             if (lossy) {
                 // the state machine of nearest_delta.go:36-42 / nearest_delta2.go:39-46, sequential by construction
                 if (lane == 0) {
@@ -159,9 +179,11 @@ __global__ void __launch_bounds__(128) k_marshal_pack(MarshalParams P) {
     for (uint32_t c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < P.ncols; c += wpg) {
         const uint32_t mt = P.mts[c];
         if (mt == 3) continue;
-        const int64_t* a = P.vals + (size_t)c * P.rows;
+        uint64_t co;
+        uint32_t n, cpb;
+        enc_col(P, c, &co, &n, &cpb);
+        const int64_t* a = P.vals + co;
         uint8_t* out = P.out + P.offs[c];
-        const uint32_t n = P.rows;
         if (mt == 2) {
             if (lane == 0) {
                 uint64_t u = zz64((int64_t)((uint64_t)a[1] - (uint64_t)a[0]));
@@ -172,10 +194,10 @@ __global__ void __launch_bounds__(128) k_marshal_pack(MarshalParams P) {
             continue;
         }
         const bool delta2 = mt == 1;
-        uint32_t pb = P.pb;
+        uint32_t pb = cpb;
         if (!delta2 && pb < 6) pb += 2;
         const bool lossy = pb < 64;
-        const int64_t* dl = lossy ? P.deltas + (size_t)c * P.rows : nullptr;
+        const int64_t* dl = lossy ? P.deltas + co : nullptr;
         uint32_t base = 0;
         for (uint32_t i0 = 1; i0 < n; i0 += 32) {
             const uint32_t i = i0 + lane;

@@ -188,6 +188,36 @@ class Part:
         return descs, payload, ids[new_series]
 
 
+def merge_parts(parts, retention_deadline=INT64_MIN, deleted_metric_ids=(), ctx=None):
+    """mergeBlockStreams (lib/storage/merge.go:19) of `parts` (a list of Part, in that order) on the GPU -> (Part, stats dict with
+    rows_count, blocks_count, min_ts, max_ts of the partHeader and the rows_merged / rows_deleted counters).  The context's dedup
+    interval applies (Context.set_dedup_interval).  deleted_metric_ids: any iterable of MetricIDs (sorted here)."""
+    ctx = ctx or _lib.default_context()
+    files = (_lib.PartFiles * max(len(parts), 1))()
+    keep = []
+    for f, p in zip(files, parts):
+        for name in ("metaindex", "index", "timestamps", "values"):
+            a = np.ascontiguousarray(getattr(p, name + "_bin"), dtype=np.uint8)
+            keep.append(a)
+            setattr(f, name, a.ctypes.data_as(_lib.u8p))
+            setattr(f, name + "_len", a.size)
+    dm = np.unique(np.asarray(list(deleted_metric_ids), dtype=np.uint64))
+    h = C.c_void_p()
+    st = _lib.MergeStats()
+    check(lib().vmb_merge_parts(ctx.h, files, len(parts), int(retention_deadline), dm.ctypes.data_as(_lib.u64p), dm.size, C.byref(h),
+                                C.byref(st)))
+    try:
+        out = _lib.PartFiles()
+        check(lib().vmb_merged_part_files(h, C.byref(out)))
+        copy = lambda ptr, n: np.ctypeslib.as_array(ptr, (n,)).copy() if n else np.zeros(0, dtype=np.uint8)
+        part = Part(copy(out.metaindex, out.metaindex_len), copy(out.index, out.index_len), copy(out.timestamps, out.timestamps_len),
+                    copy(out.values, out.values_len))
+    finally:
+        lib().vmb_merged_part_free(h)
+    stats = {k: int(getattr(st, k)) for k, _ in _lib.MergeStats._fields_}
+    return part, stats
+
+
 class Blocks:
     """compressed blocks resident in HBM (vmb_blocks)"""
 
