@@ -178,6 +178,33 @@ int vmb_merge_metaindex_frame(vmb_ctx* ctx, const uint8_t* src, size_t n, uint8_
 int vmb_merged_part_files(const vmb_merged_part* p, vmb_part_files* files);
 void vmb_merged_part_free(vmb_merged_part* p);
 
+/* ---- part flushes  ==  rawRowsMarshaler.marshalToInmemoryPart (lib/storage/raw_row.go:81) for every row set of a flush ------- */
+typedef struct {            /* one rowss[i] of partition.flushRowssToInmemoryParts (partition.go:603): n rawRows (raw_row.go:12) */
+    const uint8_t* tsids;   /* [n * 24] marshaled TSIDs (tsid.go:62: MetricGroupID, JobID, InstanceID, MetricID, big endian) */
+    const int64_t* timestamps;
+    const double* values;
+    const uint8_t* precision_bits; /* 1..64 each */
+    uint64_t n;
+} vmb_raw_rows;
+/* Turns each sets[i] into one part, out[i], byte for byte what marshalToInmemoryPart writes with the library's zstd writer in place
+ * of CompressZSTDLevel(-5); stats[i] = its partHeader, rows_merged = n, rows_deleted = 0.  All sets go through the device in one
+ * pass; the parts go to vmb_merge_parts as they are (the reference's mustMergeInmemoryParts).  Per set:
+ *   - the rows are ordered by (TSID, Timestamp) (rawRowsSort.Less raw_row.go:49), the TSID compared as its 24 marshaled bytes.
+ *     Tie rule: rows with equal (TSID, Timestamp) keep their input order (a stable sort).  The reference keeps the input order
+ *     when the set is already sorted and otherwise leaves such rows in the order of Go's unstable sort.Sort, so the two agree
+ *     whenever the input is sorted or no two rows share (TSID, Timestamp);
+ *   - a block ends where a row's MetricID differs from the MetricID of the block's first row, or at 8192 rows (raw_row.go:111);
+ *     the block takes the TSID and PrecisionBits of its first row.  Rows of one MetricID with different TSIDs can share a block,
+ *     and one MetricID can own blocks that are not adjacent;
+ *   - per block: AppendFloatToDecimal (one scale), then the ctx's dedup interval > 0: deduplicateSamplesDuringMerge, then the
+ *     columns, timestamps payload sharing, index blocks and the metaindex as vmb_merge_parts writes them.
+ * An empty set gives an empty part (no blocks, zero rows).  Errors: a NULL pointer or n >= 2^32 (VMB_ERR_INVALID_ARG), a
+ * precisionBits outside 1..64 (VMB_ERR_INVALID_ARG, as CheckPrecisionBits encoding.go:68), device memory for the whole call
+ * missing (VMB_ERR_NOMEM: about 90 bytes a row plus the encoder's scratch); every out[i] is then NULL.  Free each part with
+ * vmb_merged_part_free. */
+int vmb_parts_from_rows(vmb_ctx* ctx, const vmb_raw_rows* sets, size_t nsets, vmb_merged_part** out /* [nsets] */,
+                        vmb_merge_stats* stats /* [nsets] */);
+
 /* ---- per-call drop-ins (single column; host buffers; run on the GPU) ------------------------------------- */
 /* encoding.UnmarshalValues / UnmarshalTimestamps  encoding.go:111 / :90 (unmarshalInt64Array :173) */
 int vmb_unmarshal_int64(vmb_ctx* ctx, int64_t* dst, size_t items_count, const uint8_t* src, size_t src_len, int mt,

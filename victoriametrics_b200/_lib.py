@@ -45,6 +45,11 @@ class MergeStats(C.Structure):
                 ("rows_merged", C.c_uint64), ("rows_deleted", C.c_uint64)]
 
 
+class RawRows(C.Structure):
+    """vmb_raw_rows: one row set of a flush (n rawRows of lib/storage/raw_row.go:12 as columns)"""
+    _fields_ = [("tsids", u8p), ("timestamps", i64p), ("values", f64p), ("precision_bits", u8p), ("n", C.c_uint64)]
+
+
 class RollupCfg(C.Structure):
     """vmb_rollup_cfg == rollupConfig (rollup.go:574)"""
     _fields_ = [("func_id", C.c_int32), ("flags", C.c_uint32), ("start", C.c_int64), ("end", C.c_int64),
@@ -101,6 +106,7 @@ def lib():
         "vmb_zstd_decompress_batch": (C.c_int, [vp, u8p, u64p, sz, u8p, sz, u64p, u32p, i32p]),
         "vmb_zstd_compress_batch": (C.c_int, [vp, u8p, u64p, sz, u8p, sz, u64p]),
         "vmb_merge_parts": (C.c_int, [vp, C.POINTER(PartFiles), sz, C.c_int64, u64p, sz, C.POINTER(vp), C.POINTER(MergeStats)]),
+        "vmb_parts_from_rows": (C.c_int, [vp, C.POINTER(RawRows), sz, C.POINTER(vp), C.POINTER(MergeStats)]),
         "vmb_merged_part_files": (C.c_int, [vp, C.POINTER(PartFiles)]),
         "vmb_merged_part_free": (None, [vp]),
         "vmb_merge_metaindex_frame": (C.c_int, [vp, u8p, sz, u8p, sz, C.POINTER(sz)]),

@@ -2150,7 +2150,7 @@ extern "C" int vmb_float_to_decimal_columns(vmb_ctx* ctx, int64_t* dst, int16_t*
     CU(cudaMemcpyAsync(d_src, src, n * 8, cudaMemcpyHostToDevice, st));
     uint32_t grid = (uint32_t)((ncols + 3) / 4);
     if (grid > VMB_SMS * 16u) grid = VMB_SMS * 16u;
-    k_float_to_decimal<<<grid, 128, 0, st>>>(d_src, d_dst, d_ea, d_sc, (uint32_t)ncols, (uint32_t)rows);
+    k_float_to_decimal<<<grid, 128, 0, st>>>(d_src, d_dst, d_ea, d_sc, (uint32_t)ncols, (uint32_t)rows, nullptr, nullptr);
     count_launch(ctx);
     CU(cudaMemcpyAsync(dst, d_dst, n * 8, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(scales, d_sc, ncols * 2, cudaMemcpyDeviceToHost, st));
@@ -2159,3 +2159,4 @@ extern "C" int vmb_float_to_decimal_columns(vmb_ctx* ctx, int64_t* dst, int16_t*
     return VMB_OK;
 }
 #include "merge.inc"
+#include "flush.inc"

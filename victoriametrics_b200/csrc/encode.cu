@@ -224,21 +224,26 @@ __global__ void __launch_bounds__(128) k_marshal_pack(MarshalParams P) {
     }
 }
 
-// ---- decimal.AppendFloatToDecimal (lib/decimal/decimal.go:173-257) for many equal-length columns: one warp per column.
+// ---- decimal.AppendFloatToDecimal (lib/decimal/decimal.go:173-257) for many columns: one warp per column.
 // FromFloat per value (:437, the same code as the host encoder: marshal.inc is compiled for both sides), the minimum exponent over
 // the non-special values (:203-211), the down-shift that keeps every up-scaled mantissa inside int64 (:213-224), the rescale
 // (:231-249); the all-zeros / all-ones fast paths (:177-184) come out of the same reductions.
+// Ragged columns (the flush path): column c holds col_rows[c] values at col_off[c] of src, dst and ea; nullptr: every column holds
+// `rows` values at c * rows.
 __global__ void __launch_bounds__(128) k_float_to_decimal(const double* __restrict__ src, int64_t* __restrict__ dst, int16_t* __restrict__ ea,
-                                                          int16_t* __restrict__ scales, uint32_t ncols, uint32_t rows) {
+                                                          int16_t* __restrict__ scales, uint32_t ncols, uint32_t rows,
+                                                          const uint64_t* __restrict__ col_off, const uint32_t* __restrict__ col_rows) {
     const int lane = lane_id();
     const uint32_t wpg = gridDim.x * (blockDim.x >> 5);
     for (uint32_t c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < ncols; c += wpg) {
-        const double* f = src + (size_t)c * rows;
-        int64_t* v = dst + (size_t)c * rows;
-        int16_t* e = ea + (size_t)c * rows;
+        const size_t co = col_off ? col_off[c] : (size_t)c * rows;
+        const uint32_t n = col_off ? col_rows[c] : rows;
+        const double* f = src + co;
+        int64_t* v = dst + co;
+        int16_t* e = ea + co;
         bool zeros = true, ones = true;
         int min_exp = 32767;
-        for (uint32_t i = lane; i < rows; i += 32) {
+        for (uint32_t i = lane; i < n; i += 32) {
             const double x = f[i];
             const unsigned long long b = (unsigned long long)__double_as_longlong(x);
             zeros &= b == 0ull;
@@ -256,12 +261,12 @@ __global__ void __launch_bounds__(128) k_float_to_decimal(const double* __restri
         for (int o = 16; o; o >>= 1) min_exp = min(min_exp, __shfl_xor_sync(VMB_FULL, min_exp, o));
         __syncwarp();
         if (zeros || ones) {
-            for (uint32_t i = lane; i < rows; i += 32) v[i] = ones ? 1 : 0;
+            for (uint32_t i = lane; i < n; i += 32) v[i] = ones ? 1 : 0;
             if (lane == 0) scales[c] = 0;
             continue;
         }
         int down = 0;
-        for (uint32_t i = lane; i < rows; i += 32) {
+        for (uint32_t i = lane; i < n; i += 32) {
             const int up = (int16_t)(e[i] - min_exp);
             const int d = (int16_t)(up - vmb_host::max_up_exponent(v[i]));
             down = max(down, d);
@@ -269,7 +274,7 @@ __global__ void __launch_bounds__(128) k_float_to_decimal(const double* __restri
 #pragma unroll
         for (int o = 16; o; o >>= 1) down = max(down, __shfl_xor_sync(VMB_FULL, down, o));
         const int16_t mexp = (int16_t)(min_exp + down);
-        for (uint32_t i = lane; i < rows; i += 32) {
+        for (uint32_t i = lane; i < n; i += 32) {
             int64_t x = v[i];
             if (vmb_host::special(x)) continue;
             int adj = (int16_t)(e[i] - mexp);

@@ -188,6 +188,51 @@ class Part:
         return descs, payload, ids[new_series]
 
 
+def _take_part(h):
+    """the files of a vmb_merged_part handle as a Part (copied out), then the handle freed"""
+    try:
+        out = _lib.PartFiles()
+        check(lib().vmb_merged_part_files(h, C.byref(out)))
+        copy = lambda ptr, n: np.ctypeslib.as_array(ptr, (n,)).copy() if n else np.zeros(0, dtype=np.uint8)
+        return Part(copy(out.metaindex, out.metaindex_len), copy(out.index, out.index_len), copy(out.timestamps, out.timestamps_len),
+                    copy(out.values, out.values_len))
+    finally:
+        lib().vmb_merged_part_free(h)
+
+
+def parts_from_rows(sets, ctx=None):
+    """rawRowsMarshaler.marshalToInmemoryPart (lib/storage/raw_row.go:81) for every row set of a flush in one call on the GPU.
+    sets: [(tsids uint8 [n, 24] or [n * 24], timestamps int64 [n], values float64 [n], precision_bits uint8 [n])] ->
+    [(Part, stats dict as merge_parts gives it)], one per set.  Rows with equal (TSID, Timestamp) keep their input order.  The
+    context's dedup interval applies (Context.set_dedup_interval)."""
+    ctx = ctx or _lib.default_context()
+    rows = (_lib.RawRows * max(len(sets), 1))()
+    keep = []
+    for r, (tsids, ts, vals, pbs) in zip(rows, sets):
+        t = np.ascontiguousarray(tsids, dtype=np.uint8).reshape(-1)
+        a = np.ascontiguousarray(ts, dtype=np.int64)
+        v = np.ascontiguousarray(vals, dtype=np.float64)
+        p = np.ascontiguousarray(pbs, dtype=np.uint8)
+        if not (t.size == 24 * a.size and a.size == v.size == p.size):
+            raise ValueError("a row set needs 24 TSID bytes, a timestamp, a value and precisionBits per row")
+        keep += [t, a, v, p]
+        r.tsids, r.timestamps = t.ctypes.data_as(_lib.u8p), a.ctypes.data_as(_lib.i64p)
+        r.values, r.precision_bits, r.n = v.ctypes.data_as(_lib.f64p), p.ctypes.data_as(_lib.u8p), a.size
+    hs = (C.c_void_p * max(len(sets), 1))()
+    st = (_lib.MergeStats * max(len(sets), 1))()
+    check(lib().vmb_parts_from_rows(ctx.h, rows, len(sets), hs, st))
+    out = []
+    try:
+        for i in range(len(sets)):
+            out.append((_take_part(hs[i]), {k: int(getattr(st[i], k)) for k, _ in _lib.MergeStats._fields_}))
+            hs[i] = None
+    finally:
+        for h in hs[:len(sets)]:
+            if h:
+                lib().vmb_merged_part_free(h)
+    return out
+
+
 def merge_parts(parts, retention_deadline=INT64_MIN, deleted_metric_ids=(), ctx=None):
     """mergeBlockStreams (lib/storage/merge.go:19) of `parts` (a list of Part, in that order) on the GPU -> (Part, stats dict with
     rows_count, blocks_count, min_ts, max_ts of the partHeader and the rows_merged / rows_deleted counters).  The context's dedup
